@@ -14,6 +14,7 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 
 from oracle import pyoracle as po  # noqa: E402
+from tests import test_esdf_options_gpu as teo  # noqa: E402
 from tests import test_esdf_reference_gpu as te  # noqa: E402
 from tests import test_icp_cpu as tic  # noqa: E402
 from tests import test_icp_gpu as ti  # noqa: E402
@@ -35,6 +36,8 @@ def cases():
         out[f"merged/{name}"] = lambda lib, n=name: tm.reference_side(n, lib)[2]
     for key in te.PIN_KEYS:
         out[f"esdf/{key}"] = lambda lib, k=key: te.reference_side(k, lib)[2]
+    for key in teo.PIN_KEYS:
+        out[f"esdf_options/{key}"] = lambda lib, k=key: teo.reference_side(k, lib)[2]
     for key in tg.PIN_KEYS:
         out[f"tsdf_ground_truth/{key}"] = lambda lib, k=key: tg.reference_side(k, lib)[1]
     for key in ti.PIN_KEYS:

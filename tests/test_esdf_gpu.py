@@ -114,6 +114,12 @@ def test_update_from_tsdf_blocks_and_setters():
     eint.setFullEuclidean(True)
     omap.esdf_set_full_euclidean(True)
     assert eint.getFullEuclidean() is True
+    eint.updateFromTsdfLayerBatch()
+    omap.esdf_update(batch=True)
+    rep = compare_esdf(esdf, omap, 5.0)
+    print("full Euclidean", rep)
+    assert rep["blocks_equal"] and rep["observed_equal"] and rep["fixed_equal"] and rep["hallucinated_equal"], rep
+    assert rep["rmse"] <= 0.3 * 0.1, rep   # (the reference's own full-Euclidean result depends on its pop order)
     eint.setFullEuclidean(False)
     omap.esdf_set_full_euclidean(False)
     eint.updateFromTsdfLayerBatch()

@@ -86,13 +86,15 @@ def _gt_config(voxel):
 
 def reference_side(key, lib):
     """The oracle side of case `key` ("<room config>/<scene>" or "ground_truth/<voxel>"): the scans, the oracle
-    maps (incremental ESDF; for ground_truth also a batch one) and the digest of their TSDF and ESDF layers."""
+    maps (incremental ESDF; for ground_truth also a batch one and a full-Euclidean batch one, the three layers of
+    test_sdf_integrators.cc:183-245) and the digest of their TSDF and ESDF layers."""
     what, arg = key.split("/")
     if what == "ground_truth":
         voxel = float(arg)
         trunc, ekw = _gt_config(voxel)
         scans = _gt_scans()
         maps = [_oracle(lib, voxel, trunc, ekw, scans, batch) for batch in (False, True)]
+        maps.append(_oracle(lib, voxel, trunc, dict(ekw, full_euclidean_distance=1), scans, True))
     else:
         sc = SCENES[arg]
         ekw = dict(max_distance_m=2.0, default_distance_m=2.0, min_distance_m=sc["trunc"] / 2, **ROOM_CONFIGS[what])
@@ -196,7 +198,7 @@ def test_esdf_reference_acceptance_criteria_vs_ground_truth(voxel):
     beside it and must not be better than the device by more than a hair."""
     trunc, ekw = _gt_config(voxel)
     max_d = ekw["max_distance_m"]
-    scans, (omap, omap_b), digest = reference_side(f"ground_truth/{voxel}", pins.lib())
+    scans, (omap, omap_b, omap_fe), digest = reference_side(f"ground_truth/{voxel}", pins.lib())
     pins.check(f"esdf/ground_truth/{voxel}", digest)
     tsdf, integ, esdf_inc, e_inc = _device(voxel, trunc, ekw)
     for s in scans:
@@ -204,23 +206,33 @@ def test_esdf_reference_acceptance_criteria_vs_ground_truth(voxel):
         e_inc.updateFromTsdfLayer(True)
     inc = _gt_errors(esdf_inc.blocks(), voxel, max_d)
     ref_inc = _gt_errors(omap.blocks(1), voxel, max_d)
-    # batch, on a second ESDF layer over the same TSDF map
-    tsdf2, integ2, esdf_b, e_b = _device(voxel, trunc, ekw)
-    for s in scans:
-        integ2.integratePointCloud((s[2], s[3]), s[0], s[1])
-    e_b.updateFromTsdfLayerBatch()
-    bat = _gt_errors(esdf_b.blocks(), voxel, max_d)
+    # batch and full-Euclidean batch, on more ESDF layers over the same TSDF map
+    bat, fe = (_gt_errors(gt_batch_layer(scans, voxel, full_euclidean).blocks(), voxel, max_d)
+               for full_euclidean in (False, True))
     ref_bat = _gt_errors(omap_b.blocks(1), voxel, max_d)
+    ref_fe = _gt_errors(omap_fe.blocks(1), voxel, max_d)
     print("voxel", voxel, "device incremental", inc, "| reference incremental", ref_inc)
     print("voxel", voxel, "device batch", bat, "| reference batch", ref_bat)
-    for r in (inc, bat):
+    print("voxel", voxel, "device full-Euclidean batch", fe, "| reference full-Euclidean batch", ref_fe)
+    for r in (inc, bat, fe):
         assert r["min_error"] <= 1e-4                      # EXPECT_NEAR(min_error, 0, 1e-4)
         assert r["max_error"] < max_d                      # EXPECT_LT(max_error, esdf_max_distance_)
         assert r["rmse"] < max_d * voxel                   # EXPECT_LT(rmse, esdf_max_distance_ * voxel_size_)
-    assert inc["voxels"] == bat["voxels"]                  # EXPECT_EQ(num_overlapping_voxels)
+    assert inc["voxels"] == bat["voxels"] == fe["voxels"]  # EXPECT_EQ(num_overlapping_voxels)
     assert abs(inc["rmse"] - bat["rmse"]) <= 1e-2          # kKindaSimilar
     assert abs(inc["max_error"] - bat["max_error"]) <= 1.0  # kCloseEnough
     # and against the reference's own result on the same input
-    assert inc["voxels"] == ref_inc["voxels"] and bat["voxels"] == ref_bat["voxels"]
+    assert inc["voxels"] == ref_inc["voxels"] and bat["voxels"] == ref_bat["voxels"] and fe["voxels"] == ref_fe["voxels"]
     assert inc["rmse"] <= ref_inc["rmse"] * 1.02 + 1e-4
     assert bat["rmse"] <= ref_bat["rmse"] * 1.02 + 1e-4
+    assert fe["rmse"] <= ref_fe["rmse"] * 1.02 + 1e-4
+
+
+def gt_batch_layer(scans, voxel, full_euclidean):
+    """The device ESDF layer of a batch update (full-Euclidean or not) over the ground-truth scans."""
+    trunc, ekw = _gt_config(voxel)
+    tsdf, integ, esdf, eint = _device(voxel, trunc, dict(ekw, full_euclidean_distance=int(full_euclidean)))
+    for s in scans:
+        integ.integratePointCloud((s[2], s[3]), s[0], s[1])
+    eint.updateFromTsdfLayerBatch()
+    return esdf

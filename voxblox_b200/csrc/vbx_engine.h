@@ -49,6 +49,7 @@ enum : uint32_t {
   kErrCoordRange = 4u,      // |voxel coordinate| >= 2^20 * vps
   kErrUpdatesFull = 8u,     // ray-voxel updates exceed max_updates_per_pass
   kFatalErrors = 15u,       // any of the above
+  kErrParentRange = 16u,    // ESDF, full-Euclidean mode: a parent vector component outside [-512, 511]
   kSkipped = 32u,           // not an error: the scan was queued behind a scan that must be redone (vbx_capi.cu)
 };
 
@@ -294,6 +295,9 @@ struct vbx_ctx {
   uint32_t* esdf_seed_list = nullptr;
   float* esdf_seed_val = nullptr;
   uint32_t* esdf_touched = nullptr;
+  // full-Euclidean mode only (allocated by its first update): every voxel's distance and parent as one 64-bit
+  // word, so that the wavefront lowers both in a single atomicMin (vbx_esdf.cu, fe_pack)
+  unsigned long long* esdf_fe = nullptr;
   int esdf_grid_raise = 0, esdf_grid_lower = 0, esdf_sms = 0, esdf_ctas_wide = 1, esdf_ctas_small = 1;
   uint32_t esdf_pending_raise = 0, esdf_pending_open = 0;  // raise_ / open_ entries queued by addNewRobotPosition
   bool maybe_esdf_only = false;                            // some slot may carry kSlotNoTsdf

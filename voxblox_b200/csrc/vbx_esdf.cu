@@ -436,13 +436,47 @@ __global__ void k_esdf_raise(EsdfParams E, Tables tab, uint32_t* raise_a, uint32
   }
 }
 
+// Full-Euclidean mode: the step a source propagates is computed from its parent vector
+// (voxel_size * (|parent - dir| - |parent|), cc:414-426), so a voxel's distance and parent must change
+// together.  During the wavefront both live in one 64-bit word per voxel (vbx_ctx::esdf_fe):
+//   bits 63..32  the distance's bit pattern as a signed int (the order atomicMin uses, see the top of the file)
+//   bits 31..0   the parent, each component + 512 in 10 bits (x low)
+// so a signed 64-bit atomicMin lowers distance and parent as one unit (equal distances: the smaller parent
+// code wins, whatever the order), and a source reads a matching pair with one 64-bit load.
+constexpr int kFeBias = 512;
+__device__ __forceinline__ bool fe_parent_ok(int x, int y, int z) {
+  return x >= -kFeBias && x < kFeBias && y >= -kFeBias && y < kFeBias && z >= -kFeBias && z < kFeBias;
+}
+__device__ __forceinline__ long long fe_pack(float d, int x, int y, int z) {
+  const uint32_t code = (uint32_t)(x + kFeBias) | ((uint32_t)(y + kFeBias) << 10) | ((uint32_t)(z + kFeBias) << 20);
+  return (long long)(((unsigned long long)(uint32_t)__float_as_int(d) << 32) | code);
+}
+__device__ __forceinline__ float fe_dist(long long w) { return __int_as_float((int)(w >> 32)); }
+__device__ __forceinline__ void fe_parent(long long w, int* x, int* y, int* z) {
+  const uint32_t code = (uint32_t)w;
+  *x = (int)(code & 1023u) - kFeBias;
+  *y = (int)((code >> 10) & 1023u) - kFeBias;
+  *z = (int)((code >> 20) & 1023u) - kFeBias;
+}
+
+// full-Euclidean mode, before the wavefront: every voxel's (distance, parent) into its 64-bit word
+__global__ void k_esdf_fe_pack(Tables tab, uint64_t nvox, long long* fe, ScanState* st) {
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nvox; i += (uint64_t)gridDim.x * blockDim.x) {
+    const EsdfWords& e = reinterpret_cast<const EsdfWords*>(tab.esdf)[i];
+    if (!fe_parent_ok(e.px, e.py, e.pz)) atomicOr(&st->error, kErrParentRange);
+    fe[i] = fe_pack(e.distance, e.px, e.py, e.pz);
+  }
+}
+
 // Step (3), processOpenSet cc:371-496: wavefront relaxation.  One warp per frontier voxel, one
 // lane per neighbour; a lowered neighbour joins the next frontier (once: the in_queue flag).
 // A voxel leaves the queue (voxel->in_queue = false, cc:384) when its warp starts on it: the flag is
 // cleared BEFORE the distance is read, so a neighbour that lowers this voxel either still sees the
 // flag (then its lower value is the one read here) or re-queues the voxel for the next sweep.
+// fe: nullptr in quasi-Euclidean mode; in full-Euclidean mode the packed (distance, parent) words, which
+// stand in for the voxels' distance and parent fields until k_esdf_parents writes them back.
 __global__ void k_esdf_lower(EsdfParams E, Tables tab, uint32_t* front_a, uint32_t* front_b, uint32_t* touched_list,
-                             ScanState* st) {
+                             long long* fe, ScanState* st) {
   cg::grid_group grid = cg::this_grid();
   const int lane = threadIdx.x & 31;
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -466,7 +500,15 @@ __global__ void k_esdf_lower(EsdfParams E, Tables tab, uint32_t* front_a, uint32
       }
       __syncwarp();
       const EsdfWords* vp = vpm;
-      const float vd = *reinterpret_cast<const volatile float*>(&vp->distance);
+      float vd;
+      int vpx = 0, vpy = 0, vpz = 0;  // (full-Euclidean mode: the source's parent, read with its distance)
+      if (E.full_euclidean) {
+        const long long w = *reinterpret_cast<const volatile long long*>(&fe[ref]);
+        vd = fe_dist(w);
+        fe_parent(w, &vpx, &vpy, &vpz);
+      } else {
+        vd = *reinterpret_cast<const volatile float*>(&vp->distance);
+      }
       const uint32_t vf = *reinterpret_cast<const volatile uint32_t*>(&vp->flags);
       if (!(vf & kFlagObserved) || vd >= E.max_distance || vd <= -E.max_distance) continue;  // cc:387-390
       if (lane >= 26) continue;
@@ -476,25 +518,31 @@ __global__ void k_esdf_lower(EsdfParams E, Tables tab, uint32_t* front_a, uint32
       const uint32_t nf = *reinterpret_cast<const volatile uint32_t*>(&np->flags);
       if (!(nf & kFlagObserved) || (nf & kFlagFixed)) continue;  // cc:407-411
       float dist = nbr_dist(E, lane);
+      const int npx = vpx - kOff[lane][0], npy = vpy - kOff[lane][1], npz = vpz - kOff[lane][2];  // new_parent
       if (E.full_euclidean) {  // cc:414-426
-        const F3 npar = f3((float)(vp->px - kOff[lane][0]), (float)(vp->py - kOff[lane][1]),
-                           (float)(vp->pz - kOff[lane][2]));
-        dist = fmul(E.voxel_size, fsub(norm3(npar), norm3(f3((float)vp->px, (float)vp->py, (float)vp->pz))));
+        dist = fmul(E.voxel_size, fsub(norm3(f3((float)npx, (float)npy, (float)npz)),
+                                       norm3(f3((float)vpx, (float)vpy, (float)vpz))));
         if (dist < 0.0f) continue;
+        if (!fe_parent_ok(npx, npy, npz)) {
+          atomicOr(&st->error, kErrParentRange);
+          continue;
+        }
       }
-      const float nd = *reinterpret_cast<const volatile float*>(&np->distance);
+      const float nd = E.full_euclidean ? fe_dist(*reinterpret_cast<const volatile long long*>(&fe[nref]))
+                                        : *reinterpret_cast<const volatile float*>(&np->distance);
+      // lower the neighbour to v (with new_parent in full-Euclidean mode); true if this call changed it
+      auto lower_to = [&](float v) -> bool {
+        if (E.full_euclidean) {
+          const long long w = fe_pack(v, npx, npy, npz);
+          return atomicMin(&fe[nref], w) > w;
+        }
+        return atomicMin(reinterpret_cast<int*>(&np->distance), __float_as_int(v)) > __float_as_int(v);
+      };
       bool changed = false;
-      int* nbits = reinterpret_cast<int*>(&np->distance);
       if (vd > 0.0f && nd > 0.0f) {  // both outside, cc:429-443
-        if (fadd(fadd(vd, dist), E.min_diff) < nd) {
-          const float cand = fadd(vd, dist);
-          changed = atomicMin(nbits, __float_as_int(cand)) > __float_as_int(cand);
-        }
+        if (fadd(fadd(vd, dist), E.min_diff) < nd) changed = lower_to(fadd(vd, dist));
       } else if (vd <= 0.0f && nd <= 0.0f) {  // both inside, cc:444-457
-        if (fsub(fsub(vd, dist), E.min_diff) > nd) {
-          const float cand = fsub(vd, dist);
-          changed = atomicMin(nbits, __float_as_int(cand)) > __float_as_int(cand);
-        }
+        if (fsub(fsub(vd, dist), E.min_diff) > nd) changed = lower_to(fsub(vd, dist));
       } else {  // signs differ, cc:458-488 (incl. the sign-vs-distance comparison of cc:464)
         const float pot = fsub(vd, fmul((float)signum_d(vd), dist));
         if (fabsf(fsub(pot, nd)) > dist) {
@@ -502,22 +550,17 @@ __global__ void k_esdf_lower(EsdfParams E, Tables tab, uint32_t* front_a, uint32
           // pops first.  The device keeps the candidate nearest the surface (order free): the
           // assignment is applied only when it lowers |distance|.
           const float nv = ((float)signum_d(pot) == nd) ? pot : fmul((float)signum_d(nd), dist);
-          if ((nv > 0.0f) == (nd > 0.0f)) {
-            changed = atomicMin(nbits, __float_as_int(nv)) > __float_as_int(nv);
-          }
+          if ((nv > 0.0f) == (nd > 0.0f)) changed = lower_to(nv);
         }
       }
       if (changed) {
         atomicAdd(&st->esdf_counts[5], 1u);
         mark_mirror(tab, E.L, nref);
-        // neighbor_voxel->parent = new_parent (cc:436,450,470,481).  Written unguarded: when two
-        // sources lower the same voxel in one sweep the last writer wins; k_esdf_parents then
-        // re-derives the parent from the converged distances (quasi-Euclidean mode).
-        if (E.full_euclidean) {
-          np->px = vp->px - kOff[lane][0];
-          np->py = vp->py - kOff[lane][1];
-          np->pz = vp->pz - kOff[lane][2];
-        } else {
+        // neighbor_voxel->parent = new_parent (cc:436,450,470,481).  Full-Euclidean mode: it went into the
+        // packed word with the distance.  Quasi-Euclidean mode: written unguarded, when two sources lower the
+        // same voxel in one sweep the last writer wins; k_esdf_parents then re-derives the parent from the
+        // converged distances.
+        if (!E.full_euclidean) {
           np->px = -kOff[lane][0];
           np->py = -kOff[lane][1];
           np->pz = -kOff[lane][2];
@@ -535,14 +578,21 @@ __global__ void k_esdf_lower(EsdfParams E, Tables tab, uint32_t* front_a, uint32
 // Parent direction of every voxel the wavefront lowered (quasi-Euclidean mode): the first
 // neighbour in table order whose converged distance reproduces this voxel's distance through
 // the relaxation rule.  (The reference stores the neighbour that happened to lower it last;
-// with equal candidates that is its visiting order.)
-__global__ void k_esdf_parents(EsdfParams E, Tables tab, const uint32_t* __restrict__ touched_list, ScanState* st) {
+// with equal candidates that is its visiting order.)  Full-Euclidean mode: the distance and parent
+// the wavefront left in the voxel's packed word.
+__global__ void k_esdf_parents(EsdfParams E, Tables tab, const uint32_t* __restrict__ touched_list,
+                               const long long* __restrict__ fe, ScanState* st) {
   const uint32_t n = min(st->lowered_n, E.cap);
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const uint32_t ref = touched_list[i];
     EsdfWords* ep = reinterpret_cast<EsdfWords*>(tab.esdf) + ref;
     atomicAnd(&ep->flags, ~kBitLowered);
-    if (E.full_euclidean) continue;
+    if (E.full_euclidean) {
+      const long long w = fe[ref];
+      ep->distance = fe_dist(w);
+      fe_parent(w, &ep->px, &ep->py, &ep->pz);
+      continue;
+    }
     const float d = ep->distance;
     for (int k = 0; k < 26; ++k) {
       const uint32_t nref = neighbor_ref(tab, E.L, ref, k);
@@ -706,10 +756,11 @@ static inline unsigned int grid_for(uint64_t n, int block) { return (unsigned in
 
 int esdf_destroy(vbx_ctx* c) {
   void* ptrs[] = {c->tab.esdf, c->frontier[0], c->frontier[1], c->raise_q[0], c->raise_q[1], c->esdf_block_list,
-                  c->esdf_seed_list, c->esdf_seed_val, c->esdf_touched};
+                  c->esdf_seed_list, c->esdf_seed_val, c->esdf_touched, c->esdf_fe};
   for (void* p : ptrs) {
     if (p) cudaFree(p);
   }
+  c->esdf_fe = nullptr;
   c->tab.esdf = nullptr;
   c->frontier[0] = c->frontier[1] = c->raise_q[0] = c->raise_q[1] = c->esdf_block_list = nullptr;
   c->esdf_seed_list = c->esdf_touched = nullptr;
@@ -889,6 +940,10 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
   E.d3 = E.u3 * c->voxel_size;
   E.cap = (uint32_t)c->frontier_cap;
   uint64_t launches = 0;
+  if (E.full_euclidean && !c->esdf_fe) {
+    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_fe),
+                           (size_t)c->tab.max_blocks * c->vox_per_block * sizeof(unsigned long long)));
+  }
   VBX_CUDA(c, cudaEventRecord(c->ev0, s));
   if (c->profiling) cudaEventRecord(c->sev[0], s);
   VBX_CUDA(c, cudaMemsetAsync(c->d_state, 0, sizeof(ScanState), s));
@@ -958,11 +1013,17 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
       VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_esdf_raise, dim3(c->esdf_grid_raise), dim3(256), args, 0, s));
     }
     if (c->profiling) cudaEventRecord(c->sev[2], s);
+    long long* fe = nullptr;
+    if (E.full_euclidean) {
+      fe = reinterpret_cast<long long*>(c->esdf_fe);
+      k_esdf_fe_pack<<<c->grid_sms * 8, 256, 0, s>>>(c->tab, (uint64_t)c->n_blocks * c->vox_per_block, fe, c->d_state);
+      launches += 1;
+    }
     {
-      void* args[] = {&E, &c->tab, &c->frontier[0], &c->frontier[1], &c->esdf_touched, &c->d_state};
+      void* args[] = {&E, &c->tab, &c->frontier[0], &c->frontier[1], &c->esdf_touched, &fe, &c->d_state};
       VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_esdf_lower, dim3(c->esdf_grid_lower), dim3(256), args, 0, s));
     }
-    k_esdf_parents<<<c->grid_sms * 8, 256, 0, s>>>(E, c->tab, c->esdf_touched, c->d_state);
+    k_esdf_parents<<<c->grid_sms * 8, 256, 0, s>>>(E, c->tab, c->esdf_touched, fe, c->d_state);
     if (c->profiling) cudaEventRecord(c->sev[3], s);
     launches += 3;
     if (nb > 0 && !batch && clear_updated_flag) {
@@ -985,6 +1046,9 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
     }
   }
   if (c->h_state->error & kErrUpdatesFull) return fail(c, VBX_E_CAPACITY, "ESDF wavefront queue capacity exceeded");
+  if (c->h_state->error & kErrParentRange) {
+    return fail(c, VBX_E_CAPACITY, "full-Euclidean ESDF: a parent vector component left [-512, 511] voxels");
+  }
   for (int i = 0; i < 7; ++i) c->esdf_counters[i] = c->h_state->esdf_counts[i];
   c->esdf_counters[7] = launches;
   c->launches += launches;
