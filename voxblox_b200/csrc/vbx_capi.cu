@@ -142,6 +142,9 @@ void select_set(vbx_ctx* c, int k) {
     c->ckeys[i] = S.ckeys[i];
     c->cvals[i] = S.cvals[i];
   }
+  c->long_list = S.long_list;
+  c->long_end = S.long_end;
+  c->keep_bits = S.keep_bits;
   c->sort_plan[1] = S.sort_plan1;
   c->sort_status[1] = S.sort_status1;
 }
@@ -367,11 +370,7 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
   }
   CK(dmalloc(&c->long_list, (size_t)(c->max_updates / 32 + 1)));
   CK(dmalloc(&c->long_end, (size_t)(c->max_updates / 32 + 1)));
-  CK(dmalloc(&c->long_state, (size_t)(c->max_updates / 32 + 1)));
-  CK(dmalloc(&c->verify_run, (size_t)(c->max_updates / 32 + 1)));
-  CK(dmalloc(&c->verify_start, (size_t)(c->max_updates / 32 + 1)));
-  CK(dmalloc(&c->rec_sdf, (size_t)c->max_updates));
-  CK(dmalloc(&c->rec_w, (size_t)c->max_updates));
+  CK(dmalloc(&c->keep_bits, (size_t)(c->max_updates / 32 + 1)));
   CK(dmalloc(&c->ray_p, np));
   CK(dmalloc(&c->ray_c, np));
   CK(dmalloc(&c->ray_a, np));
@@ -419,6 +418,9 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
       a.ckeys[i] = c->ckeys[i];
       a.cvals[i] = c->cvals[i];
     }
+    a.long_list = c->long_list;
+    a.long_end = c->long_end;
+    a.keep_bits = c->keep_bits;
     a.sort_plan1 = c->sort_plan[1];
     a.sort_status1 = c->sort_status[1];
     vbx_ctx::FrontLane& f = c->lane[0];
@@ -503,6 +505,9 @@ int ensure_async(vbx_ctx* c) {
       CK(dmalloc(&S.ckeys[i], (size_t)c->max_updates));
       CK(dmalloc(&S.cvals[i], (size_t)c->max_updates));
     }
+    CK(dmalloc(&S.long_list, (size_t)(c->max_updates / 32 + 1)));
+    CK(dmalloc(&S.long_end, (size_t)(c->max_updates / 32 + 1)));
+    CK(dmalloc(&S.keep_bits, (size_t)(c->max_updates / 32 + 1)));
     CK(dmalloc(&S.sort_plan1, 1));
     CK(dmalloc(&S.sort_status1, (size_t)4 * c->sort_tiles_cap[1] * kRadix));
   }
@@ -542,8 +547,8 @@ void vbx_destroy(vbx_ctx* c) {
                   c->ckeys[1],    c->cvals[0],   c->cvals[1],    c->order,      c->ray_p,    c->ray_c,
                   c->cnt,         c->off,        c->set_start,  c->set_observed, c->d_state,
                   c->ray_list,    c->head_list,  c->long_list,  c->ray_a,      c->sort_plan[0], c->sort_plan[1],
-                  c->sort_status[0], c->sort_status[1], c->scan_status, c->long_end, c->long_state,
-                  c->verify_run,  c->verify_start, c->rec_sdf, c->rec_w, c->d_nblocks, c->order_inv, c->d_hold};
+                  c->sort_status[0], c->sort_status[1], c->scan_status, c->long_end, c->keep_bits,
+                  c->d_nblocks, c->order_inv, c->d_hold};
   for (void* p : ptrs) {
     if (p) cudaFree(p);
   }
@@ -555,7 +560,8 @@ void vbx_destroy(vbx_ctx* c) {
     vbx_ctx::ScratchSet& S = c->set[k];
     if (k > 0) {
       void* sp[] = {S.ray_p, S.ray_a, S.ray_c, S.ray_list, S.head_list, S.touched_list, S.cnt, S.off, S.d_state, S.d_xyz, S.d_rgba, S.pkeys0,
-                    S.ckeys[0], S.ckeys[1], S.cvals[0], S.cvals[1], S.sort_plan1, S.sort_status1};
+                    S.ckeys[0], S.ckeys[1], S.cvals[0], S.cvals[1], S.long_list, S.long_end, S.keep_bits,
+                    S.sort_plan1, S.sort_status1};
       for (void* p : sp) {
         if (p) cudaFree(p);
       }

@@ -73,8 +73,8 @@ struct ScanState {
   uint32_t seed_n;           // ESDF: new free voxels waiting for updateVoxelFromNeighbors
   uint32_t lowered_n;        // ESDF: voxels lowered by the wavefront
   uint32_t n_ray_list;       // bundle heads (Merged)
-  uint32_t n_long;           // voxel runs handed to k_apply_long
-  uint32_t n_verify;         // work items of k_apply_verify
+  uint32_t n_long;           // voxel runs longer than kShortRun updates (k_apply_prep's long-run list)
+  uint32_t long_ticket;      // k_apply: long runs handed out
   uint32_t n_refold;         // bundles folded a second time with IEEE division (diagnostic)
   uint32_t refold_members;   // ... and the points they hold
   uint32_t frontier_n2;      // third wavefront counter
@@ -89,7 +89,8 @@ struct ScanState {
   uint32_t n_touch_ids;      // touched-block ids handed out (>= n_touched: ids lost to a race stay unused)
   uint32_t rec_key_bits;     // bits an update-record key uses: voxel-in-block bits + bits of the touched ids
   uint32_t esdf_ticket[6];   // ESDF queue kernels: work hand-out counters, rotating like the queue counters ([0..2] raise, [3..5] lower)
-  uint32_t reserved[15];
+  uint32_t tile_ticket;      // k_apply: record tiles of the short runs handed out
+  uint32_t reserved[14];
 };
 static_assert(sizeof(ScanState) == 256, "the status block the host reads back is 256 bytes");
 
@@ -176,13 +177,9 @@ struct vbx_ctx {
   vbx::OrderScratch order_scratch{};         // k_bundle_order's global tables (front-lane private)
   vbx::RehashSchedule rehash{};            // libstdc++'s unordered_map growth schedule (vbx_create)
   size_t order_smem_bytes = 0;             // dynamic shared memory of k_bundle_order
-  unsigned long long* long_list = nullptr; // [max_updates / 32 + 1] starts of long voxel runs
-  unsigned long long* long_end = nullptr;
-  uint32_t* long_state = nullptr;
-  uint32_t* verify_run = nullptr;          // [max_updates / 32 + 1] work items of k_apply_verify
-  unsigned long long* verify_start = nullptr;
-  float* rec_sdf = nullptr;                // [max_updates] per sorted record
-  float* rec_w = nullptr;
+  unsigned long long* long_list = nullptr; // [max_updates / 32 + 1] first record of each long voxel run (hand-off set private)
+  unsigned long long* long_end = nullptr;  // [max_updates / 32 + 1] one past its last record
+  uint32_t* keep_bits = nullptr;           // [max_updates / 32 + 1] per sorted record: the update keeps (+T, max_weight)
   float4* ray_p = nullptr;    // point_G.xyz, flags (bit 0: clearing ray)
   float4* ray_a = nullptr;    // point_G - origin, |point_G - origin|
   uint2* ray_c = nullptr;     // colour, weight bits
@@ -229,6 +226,9 @@ struct vbx_ctx {
     uint64_t* pkeys0 = nullptr;  // sorted bundle keys (read again by the ray walk)
     uint32_t* ckeys[2] = {nullptr, nullptr};  // update records (written by the walk, read by apply)
     uint32_t* cvals[2] = {nullptr, nullptr};
+    unsigned long long* long_list = nullptr;  // long voxel runs and keep bits of the sorted records (k_apply_prep -> k_apply)
+    unsigned long long* long_end = nullptr;
+    uint32_t* keep_bits = nullptr;
     vbx::SortPlan* sort_plan1 = nullptr;
     uint32_t* sort_status1 = nullptr;
     cudaEvent_t copy_done = nullptr, front_done = nullptr, walked = nullptr, sorted = nullptr, back_done = nullptr;

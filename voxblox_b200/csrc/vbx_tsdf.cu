@@ -16,10 +16,13 @@
 //   k_rays_emit      second DDA walk writing (voxel id, ray id) records
 //   sort             stable radix sort by voxel id: every voxel's updates become one
 //                    run, ordered by ray rank
-//   k_apply_short /  updateTsdfVoxel (cc:150-209) applied sequentially per voxel --
-//   k_apply_long     clamp-after-every-update semantics preserved exactly, with no
-//                    locks and no atomics on voxels.  Runs longer than 32 updates
-//                    (free space near the sensor) continue in a warp-per-run kernel.
+//   k_apply_prep     per sorted record: sdf, weight, colour and a keep bit; the list
+//                    of runs longer than 32 updates -- no voxel is read, so it runs
+//                    on the sort stream
+//   k_apply          updateTsdfVoxel (cc:150-209) applied sequentially per voxel --
+//                    clamp-after-every-update semantics preserved exactly, with no
+//                    locks and no atomics on voxels.  A warp per long run (free space
+//                    near the sensor), then a thread per short run.
 //
 // Update order.  The reference applies a voxel's updates in whatever order its
 // threads reach the voxel's mutex (cc:186); with one thread that is point order for
@@ -29,6 +32,7 @@
 // of the reference's libstdc++ unordered_map (k_bundle_order, vbx_order.cuh), normal
 // bundles before clearing bundles (cc:323-335).  See DESIGN.md "update order".
 #include <algorithm>
+#include <cassert>
 #include <chrono>
 #include <cstdio>
 #include <cstring>
@@ -45,7 +49,7 @@ namespace cg = cooperative_groups;
 
 namespace vbx {
 
-constexpr int kShortRun = 32;  // updates a single thread applies before handing the run to a warp
+constexpr int kShortRun = 32;  // a voxel run of at most this many updates is applied by one thread, a longer one by a warp
 
 struct ScanParams {
   Pose T;
@@ -1185,7 +1189,8 @@ __global__ void k_pass_begin(ScanState* st, unsigned long long pass_updates) {
   st->total_updates = st->error ? 0ull : pass_updates;
   st->n_new = 0;
   st->n_long = 0;
-  st->n_verify = 0;
+  st->long_ticket = 0;
+  st->tile_ticket = 0;
 }
 
 // First kernel of an asynchronously submitted scan's back half (walk stream: submission order).
@@ -1492,209 +1497,196 @@ __device__ __forceinline__ float sdf_from(F3 vo, float4 ra) {
 // which buffer holds the result and how many records there are; with the engine's own sort both
 // live in device memory (SortPlan::final_buf, ScanState::total_updates).
 struct RecordView {
-  const uint32_t* keys[2];
-  const uint32_t* vals[2];
+  uint32_t* keys[2];
+  uint32_t* vals[2];
   const SortPlan* plan;                 // nullptr: buffer 0 holds the sorted records
   const unsigned long long* d_total;    // nullptr: total_fixed
   unsigned long long total_fixed;
 };
-__device__ __forceinline__ void open_records(const RecordView& rv, const uint32_t** ckeys, const uint32_t** cvals,
-                                             unsigned long long* total) {
-  const uint32_t sel = rv.plan ? rv.plan->final_buf : 0u;
-  *ckeys = rv.keys[sel];
-  *cvals = rv.vals[sel];
-  *total = rv.d_total ? *rv.d_total : rv.total_fixed;
-}
 
-// Voxel runs longer than kShortRun updates.  state: 0 = apply sequentially (k_apply_long),
-// 1 = candidate for the parallel fixed-point check, |2 = the check failed.
-constexpr unsigned long long kVerifyItem = 256;  // 8 records per lane: short dependent chains, many items
+// What k_apply_prep hands to k_apply besides the records themselves: the voxel runs longer than
+// kShortRun updates and one keep bit per record.  Both are private to the scan's hand-off set.
+constexpr int kApplyTile = 256;  // records per work item of k_apply's short-run phase
+constexpr int kApplyWarps = 4;   // warps per thread block of k_apply
 struct LongRuns {
-  unsigned long long* start;   // first record after the prefix the head thread applied
-  unsigned long long* end;     // one past the run's last record (state != 0)
-  uint32_t* state;
-  uint32_t* item_run;          // work items of k_apply_verify
-  unsigned long long* item_start;
-  float* rec_sdf;              // per sorted record: sdf and effective weight, written by
-  float* rec_w;                // k_apply_short's parallel phase, read by the long-run kernels
+  unsigned long long* start;   // [n_long] first record of the run
+  unsigned long long* end;     // [n_long] one past its last record
+  uint32_t* keep;              // bit j of word j / 32: record j's update maps (+T, max_weight) onto itself
+  unsigned long long cap;      // entries of start / end and words of keep: max_updates / 32 + 1
 };
 
-// One warp per work item: do all updates in [start, start + kVerifyItem) of a saturated voxel's
-// run map (+T, max_weight) onto itself?  An update does when its sdf >= T (no colour blend), the
-// new distance clamps back to +T and the weight clamps back to max_weight -- evaluated with the
-// reference's own arithmetic, so "unchanged" is exact, not approximate.
-__global__ void k_apply_verify(ScanParams P, Tables tab, RecordView rv, const float4* __restrict__ ray_a,
-                               const uint2* __restrict__ ray_c, LongRuns lr, const ScanState* st) {
-  const uint32_t* ckeys;
-  const uint32_t* cvals;
+// The prepared form of the sorted records.  After the sort only one of the two buffer pairs holds
+// records; k_apply_prep writes each record's sdf and weight into the other pair and its colour over
+// its ray id, so no buffer is added and everything stays private to the scan.
+struct Prepared {
+  const uint32_t* key;
+  const float* sdf;
+  const float* w;
+  const uint32_t* col;
   unsigned long long total;
-  open_records(rv, &ckeys, &cvals, &total);
-  if (st->error & kFatalErrors) return;
-  const int lane = threadIdx.x & 31;
-  const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint32_t n_warps = (gridDim.x * blockDim.x) >> 5;
-  const uint32_t n_items = st->n_verify;
-  const float T = P.up.trunc, W = P.up.max_weight;
-  for (uint32_t it = warp; it < n_items; it += n_warps) {
-    const uint32_t q = lr.item_run[it];
-    const unsigned long long a = lr.item_start[it];
-    const unsigned long long b = min(a + kVerifyItem, lr.end[q]);
-    bool ok = true;
-#pragma unroll
-    for (int k = 0; k < (int)(kVerifyItem / 32); ++k) {
-      const unsigned long long j = a + lane + 32ull * k;
-      if (j >= b) continue;
-      const float sdf = lr.rec_sdf[j], w = lr.rec_w[j];
-      const float nw = fadd(W, w);
-      bool keeps = sdf >= T && !(nw < VBX_EPS) && !(nw < W);
-      if (keeps) {
-        const float ns = fdiv(fadd(fmul(sdf, w), fmul(T, W)), nw);
-        keeps = (ns > 0.0f) && !(ns < T);
-      }
-      ok = ok && keeps;
-    }
-    if (!__all_sync(0xffffffffu, ok) && lane == 0) atomicOr(&lr.state[q], 2u);
-  }
+};
+__device__ __forceinline__ Prepared open_prepared(const RecordView& rv) {
+  const uint32_t sel = rv.plan ? rv.plan->final_buf : 0u;
+  Prepared r;
+  r.key = rv.keys[sel];
+  r.sdf = reinterpret_cast<const float*>(rv.keys[sel ^ 1u]);
+  r.w = reinterpret_cast<const float*>(rv.vals[sel ^ 1u]);
+  r.col = rv.vals[sel];
+  r.total = rv.d_total ? *rv.d_total : rv.total_fixed;
+  return r;
 }
 
-// One thread per run head applies the first kShortRun updates of its voxel in order
-// (updateTsdfVoxel, cc:150-209); longer runs are queued for k_apply_long.
-__global__ void __launch_bounds__(256)
-k_apply_short(ScanParams P, Tables tab, RecordView rv, const float4* __restrict__ ray_a,
-              const uint2* __restrict__ ray_c, LongRuns lr, ScanState* st) {
-  // Phase 1 (every thread): one record each -- gather its ray, form sdf and weight.  This is the
-  // expensive, perfectly parallel part; results are staged in shared memory.
-  // Phase 2 (run heads): the read-modify-write chain of updateTsdfVoxel over the staged values.
-  __shared__ uint32_t s_key[256];
-  __shared__ float s_sdf[256];
-  __shared__ float s_w[256];
-  __shared__ uint32_t s_col[256];
-  const uint32_t* ckeys;
-  const uint32_t* cvals;
-  unsigned long long total;
-  open_records(rv, &ckeys, &cvals, &total);
+// The per-record half of the apply; it reads no voxel, so it runs on the sort stream, beside the
+// previous scan's apply.  One thread per sorted record: gather its ray, form sdf, weight and colour
+// exactly as updateTsdfVoxel will use them (cc:150-209), and set its keep bit.  The bit is set when
+// the update maps a voxel at (+T, max_weight) onto itself: sdf >= T (no colour blend), the new
+// distance clamps back to +T and the weight back to max_weight -- the reference's own arithmetic,
+// so "unchanged" is exact, not approximate.  Run heads count the distinct voxels (U) and list the
+// runs longer than kShortRun updates with their [start, end).  Records of blocks this rank does not
+// own (kSkipRecord) sort to the end and are skipped.
+__global__ void __launch_bounds__(256, 6)
+k_apply_prep(ScanParams P, Tables tab, RecordView rv, const float4* __restrict__ ray_a,
+             const uint2* __restrict__ ray_c, LongRuns lr, ScanState* st) {
+  const uint32_t sel = rv.plan ? rv.plan->final_buf : 0u;
+  const uint32_t* __restrict__ keys = rv.keys[sel];
+  uint32_t* __restrict__ vals = rv.vals[sel];
+  float* __restrict__ rec_sdf = reinterpret_cast<float*>(rv.keys[sel ^ 1u]);
+  float* __restrict__ rec_w = reinterpret_cast<float*>(rv.vals[sel ^ 1u]);
+  const unsigned long long total = rv.d_total ? *rv.d_total : rv.total_fixed;
   if (st->error & kFatalErrors) return;
+  const float T = P.up.trunc, W = P.up.max_weight;
   const unsigned long long n_tiles = (total + 255ull) / 256ull;
   for (unsigned long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const unsigned long long base = tile * 256ull;
-    const unsigned long long e = base + threadIdx.x;
-    bool head = false;
-    uint32_t key = 0xffffffffu;
-    VoxelRef vr;
-    vr.ptr = nullptr;
-    vr.vo = f3(0.f, 0.f, 0.f);
-    if (e < total) key = ckeys[e];
-    if (key != kSkipRecord) {  // (records of blocks this rank does not own sort to the end and are skipped)
-      head = (e == 0) || (ckeys[e - 1] != key);
-      const uint32_t r = cvals[e];
+    const unsigned long long e = tile * 256ull + threadIdx.x;
+    const uint32_t key = e < total ? keys[e] : kSkipRecord;
+    bool keep = false, head = false;
+    if (key != kSkipRecord) {
+      const uint32_t r = vals[e];
       const float4 ra = ray_a[r];
       const uint2 rc = ray_c[r];
-      vr = locate_voxel(P, tab, key);
+      const VoxelRef vr = locate_voxel(P, tab, key);
       const float sdf = sdf_from(vr.vo, ra);
       const float w = update_weight(sdf, __uint_as_float(rc.y), P.up);
-      s_sdf[threadIdx.x] = sdf;
-      s_w[threadIdx.x] = w;
-      s_col[threadIdx.x] = rc.x;
-      lr.rec_sdf[e] = sdf;
-      lr.rec_w[e] = w;
-    }
-    s_key[threadIdx.x] = key;
-    __syncthreads();
-    head = head && vr.ptr != nullptr;
-    if (head) {
-      TsdfVoxel v = *vr.ptr;
-      unsigned long long j = e;
-      int k = 0;
-      // inside this tile: staged values
-      for (; k < kShortRun && j < base + 256ull && s_key[j - base] == key; ++k, ++j) {
-        apply_update(v, s_sdf[j - base], s_w[j - base], s_col[j - base], P.up);
+      rec_sdf[e] = sdf;
+      rec_w[e] = w;
+      vals[e] = rc.x;
+      const float nw = fadd(W, w);
+      keep = sdf >= T && !(nw < VBX_EPS) && !(nw < W);
+      if (keep) {
+        const float ns = fdiv(fadd(fmul(sdf, w), fmul(T, W)), nw);
+        keep = (ns > 0.0f) && !(ns < T);
       }
-      // a run that crosses the tile boundary continues from global memory
-      if (j == base + 256ull) {
-        for (; k < kShortRun && j < total && ckeys[j] == key; ++k, ++j) {
-          const uint32_t r = cvals[j];  // (the next tile's staged values are not visible here)
-          const float sdf = sdf_from(vr.vo, ray_a[r]);
-          const uint2 rc = ray_c[r];
-          apply_update(v, sdf, update_weight(sdf, __uint_as_float(rc.y), P.up), rc.x, P.up);
+      // (a block that found no pool slot has no voxel to update: kErrPoolFull stops the next scan's apply)
+      head = (e == 0 || keys[e - 1] != key) && vr.ptr != nullptr;
+      if (head && e + kShortRun < total && keys[e + kShortRun] == key) {
+        // the first record past the run: galloping from the record known to be in it, then bisection
+        unsigned long long lo = e + kShortRun + 1, step = 2 * kShortRun;
+        while (e + step < total && keys[e + step] == key) {
+          lo = e + step + 1;
+          step *= 2;
         }
-      }
-      *vr.ptr = v;
-      if (j < total && ckeys[j] == key) {
+        unsigned long long hi = min(e + step, total);
+        while (lo < hi) {
+          const unsigned long long mid = (lo + hi) >> 1;
+          if (keys[mid] <= key) {
+            lo = mid + 1;
+          } else {
+            hi = mid;
+          }
+        }
         const uint32_t q = atomicAdd(&st->n_long, 1u);
-        lr.start[q] = j;
-        // A voxel resting at (+T, max_weight) -- free space seen many times -- stays there as
-        // long as every remaining update maps that state onto itself, which can be checked
-        // record by record, in parallel (k_apply_verify).  Find the end of the run (records are
-        // sorted) and cut it into work items.
-        const bool saturated = v.distance == P.up.trunc && v.weight == P.up.max_weight && P.up.max_weight >= VBX_EPS;
-        uint32_t state = 0u;
-        if (saturated) {
-          unsigned long long lo = j, hi = total;  // first record past the run
-          while (lo < hi) {
-            const unsigned long long mid = (lo + hi) >> 1;
-            if (ckeys[mid] <= key) {
-              lo = mid + 1;
-            } else {
-              hi = mid;
-            }
-          }
-          lr.end[q] = lo;
-          for (unsigned long long a = j; a < lo; a += kVerifyItem) {
-            const uint32_t it = atomicAdd(&st->n_verify, 1u);
-            lr.item_run[it] = q;
-            lr.item_start[it] = a;
-          }
-          state = 1u;
-        }
-        lr.state[q] = state;
+        assert(q < lr.cap);
+        lr.start[q] = e;
+        lr.end[q] = lo;
       }
     }
-    const unsigned b = __ballot_sync(0xffffffffu, head);
-    if ((threadIdx.x & 31) == 0 && b) atomicAdd(&st->n_voxels, (uint32_t)__popc(b));
-    __syncthreads();  // the staging arrays are reused by the next tile
+    const unsigned kb = __ballot_sync(0xffffffffu, keep);
+    const unsigned hb = __ballot_sync(0xffffffffu, head);
+    if ((threadIdx.x & 31) == 0) {
+      if (e < total) {
+        assert((e >> 5) < lr.cap);
+        lr.keep[e >> 5] = kb;
+      }
+      if (hb) atomicAdd(&st->n_voxels, (uint32_t)__popc(hb));
+    }
   }
 }
 
-// One warp per long run.  32 updates are prefetched per step (records coalesced, ray data
-// gathered, sdf and weight computed in parallel); the read-modify-write chain is then
-// evaluated in order.  Free space far in front of any surface is the common long run:
-// there every update has sdf >= T and the voxel already sits at +T, so after computing the
-// exact sequential weight chain each lane checks that ITS update maps +T to +T; if all do,
-// the sequential result is (+T, chained weight) without walking the distance chain.
-__global__ void k_apply_long(ScanParams P, Tables tab, RecordView rv, const float4* __restrict__ ray_a,
-                             const uint2* __restrict__ ray_c, LongRuns lr, const ScanState* st) {
-  const uint32_t* ckeys;
-  const uint32_t* cvals;
-  unsigned long long total;
-  open_records(rv, &ckeys, &cvals, &total);
+// The first record p of [start, end) such that every record of [p, end) keeps (+T, max_weight):
+// one warp reads the keep bits from the end of the run backwards, 32 words per step.
+__device__ __forceinline__ unsigned long long keep_suffix(const uint32_t* __restrict__ keep, unsigned long long start,
+                                                          unsigned long long end, int lane) {
+  const long long w0 = (long long)(start >> 5), w1 = (long long)((end - 1) >> 5);
+  for (long long top = w1; top >= w0; top -= 32) {
+    const long long wi = top - lane;
+    uint32_t bad = 0u;
+    if (wi >= w0) {
+      uint32_t m = 0xffffffffu;
+      if (wi == w0) m &= 0xffffffffu << (start & 31u);
+      if (wi == w1) m &= 0xffffffffu >> (31u - ((end - 1) & 31u));
+      bad = ~keep[wi] & m;
+    }
+    const unsigned b = __ballot_sync(0xffffffffu, bad != 0u);
+    if (b) {
+      const int src = __ffs(b) - 1;  // the lowest lane holds the highest word with a record that does not keep
+      const uint32_t bw = __shfl_sync(0xffffffffu, bad, src);
+      return (unsigned long long)(top - src) * 32ull + (unsigned long long)(31 - __clz(bw)) + 1ull;
+    }
+  }
+  return start;
+}
+
+// The read-modify-write chains of updateTsdfVoxel (cc:150-209), applied sequentially per voxel --
+// clamp-after-every-update semantics preserved exactly, with no locks and no atomics on voxels --
+// over the records k_apply_prep prepared.  Warps first take the long runs by ticket, so the longest
+// chains start at once; then they take kApplyTile-record tiles of the short runs, one thread per
+// run.  Every voxel has exactly one owner and no warp waits on another.
+//
+// A long run is one warp's from its first record.  kG x 32 records are loaded per step (and the next
+// step's are prefetched) so that the loads of a step are all in flight together.  Free space far in
+// front of any surface is the common long run: there every update has sdf >= T and the voxel already
+// sits at +T, so after computing the exact sequential weight chain each lane checks that ITS update
+// maps +T to +T; if all do, the sequential result is (+T, chained weight) without walking the
+// distance chain.  Once the voxel rests at (+T, max_weight) and every remaining record's keep bit is
+// set, the rest of the run leaves it unchanged and is skipped.
+__global__ void __launch_bounds__(32 * kApplyWarps, 8)
+k_apply(ScanParams P, Tables tab, RecordView rv, LongRuns lr, ScanState* st) {
+  const Prepared pr = open_prepared(rv);
   if (st->error & kFatalErrors) return;
+  const uint32_t* __restrict__ keys = pr.key;
+  const float* __restrict__ rec_sdf = pr.sdf;
+  const float* __restrict__ rec_w = pr.w;
+  const uint32_t* __restrict__ rec_col = pr.col;
+  const unsigned long long total = pr.total;
   const int lane = threadIdx.x & 31;
-  const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint32_t n_warps = (gridDim.x * blockDim.x) >> 5;
   const uint32_t n_long = st->n_long;
   const float T = P.up.trunc;
-  for (uint32_t q = warp; q < n_long; q += n_warps) {
-    if (lr.state[q] == 1u) continue;  // verified: every remaining update keeps (+T, max_weight)
-    unsigned long long j0 = lr.start[q];
-    const uint32_t key = ckeys[j0];
-    const VoxelRef vr = locate_voxel(P, tab, key);
+  const bool can_rest = P.up.max_weight >= VBX_EPS;
+  for (;;) {
+    uint32_t q = 0;
+    if (lane == 0) q = atomicAdd(&st->long_ticket, 1u);
+    q = __shfl_sync(0xffffffffu, q, 0);
+    if (q >= n_long) break;
+    const unsigned long long start = lr.start[q], end = lr.end[q];
+    const VoxelRef vr = locate_voxel(P, tab, keys[start]);
     TsdfVoxel v = *vr.ptr;
-    bool done = false;
-    // sdf and weight of every record were computed by k_apply_short's parallel phase; the chain
-    // only streams them.  Four 32-record chunks are loaded per step (and the next four are
-    // prefetched) so that the loads of a step are all in flight together; colours are gathered
-    // on the rare chunks that need the full update.
+    unsigned long long keep_from = ~0ull;  // found on first need
+    unsigned long long j0 = start;
     constexpr int kG = 4;
     bool in_n[kG];
     float sdf_n[kG], w_n[kG];
 #pragma unroll
     for (int g = 0; g < kG; ++g) {
       const unsigned long long j = j0 + 32ull * g + lane;
-      in_n[g] = j < total && ckeys[j] == key;
-      sdf_n[g] = in_n[g] ? lr.rec_sdf[j] : 0.f;
-      w_n[g] = in_n[g] ? lr.rec_w[j] : 0.f;
+      in_n[g] = j < end;
+      sdf_n[g] = in_n[g] ? rec_sdf[j] : 0.f;
+      w_n[g] = in_n[g] ? rec_w[j] : 0.f;
     }
-    while (!done) {
+    for (;;) {
+      if (can_rest && v.distance == T && v.weight == P.up.max_weight) {
+        if (keep_from == ~0ull) keep_from = keep_suffix(lr.keep, start, end, lane);
+        if (j0 >= keep_from) break;
+      }
       bool in_c[kG];
       float sdf_c[kG], w_c[kG];
 #pragma unroll
@@ -1703,14 +1695,14 @@ __global__ void k_apply_long(ScanParams P, Tables tab, RecordView rv, const floa
         sdf_c[g] = sdf_n[g];
         w_c[g] = w_n[g];
       }
-      const bool more = __all_sync(0xffffffffu, in_c[kG - 1]);  // the run may continue past these records
+      const bool more = j0 + 32ull * kG < end;
       if (more) {
 #pragma unroll
         for (int g = 0; g < kG; ++g) {
           const unsigned long long j = j0 + 32ull * (kG + g) + lane;
-          in_n[g] = j < total && ckeys[j] == key;
-          sdf_n[g] = in_n[g] ? lr.rec_sdf[j] : 0.f;
-          w_n[g] = in_n[g] ? lr.rec_w[j] : 0.f;
+          in_n[g] = j < end;
+          sdf_n[g] = in_n[g] ? rec_sdf[j] : 0.f;
+          w_n[g] = in_n[g] ? rec_w[j] : 0.f;
         }
       }
       // The common long run -- free space far in front of any surface, the voxel already at +T -- is decided
@@ -1860,7 +1852,7 @@ __global__ void k_apply_long(ScanParams P, Tables tab, RecordView rv, const floa
         if (fast) {
           v.weight = w_end;
         } else {
-          const uint32_t col = in ? ray_c[cvals[j0 + 32ull * g + lane]].x : 0u;
+          const uint32_t col = in ? rec_col[j0 + 32ull * g + lane] : 0u;
           for (int k = 0; k < cnt; ++k) {
             apply_update(v, __shfl_sync(0xffffffffu, sdf, k), __shfl_sync(0xffffffffu, w, k),
                          __shfl_sync(0xffffffffu, col, k), P.up);
@@ -1868,9 +1860,67 @@ __global__ void k_apply_long(ScanParams P, Tables tab, RecordView rv, const floa
         }
       }
       j0 += 32ull * kG;
-      if (!more) done = true;
+      if (!more) break;
     }
     if (lane == 0) *vr.ptr = v;
+  }
+  // The short runs.  A warp stages its tile's records in shared memory (all loads in flight together),
+  // lists the tile's run heads, and gives each lane a head: the tile's chains run side by side.
+  __shared__ uint32_t s_key[kApplyWarps][kApplyTile];
+  __shared__ float s_sdf[kApplyWarps][kApplyTile];
+  __shared__ float s_w[kApplyWarps][kApplyTile];
+  __shared__ uint32_t s_col[kApplyWarps][kApplyTile];
+  __shared__ uint8_t s_head[kApplyWarps][kApplyTile];
+  const int wb = threadIdx.x >> 5;
+  const uint32_t n_tiles = (uint32_t)((total + kApplyTile - 1) / kApplyTile);
+  for (;;) {
+    uint32_t t = 0;
+    if (lane == 0) t = atomicAdd(&st->tile_ticket, 1u);
+    t = __shfl_sync(0xffffffffu, t, 0);
+    if (t >= n_tiles) break;
+    const unsigned long long base = (unsigned long long)t * kApplyTile;
+#pragma unroll
+    for (int s = 0; s < kApplyTile / 32; ++s) {
+      const int o = 32 * s + lane;
+      const bool in = base + o < total;
+      s_key[wb][o] = in ? keys[base + o] : kSkipRecord;
+      s_sdf[wb][o] = in ? rec_sdf[base + o] : 0.f;
+      s_w[wb][o] = in ? rec_w[base + o] : 0.f;
+      s_col[wb][o] = in ? rec_col[base + o] : 0u;
+    }
+    __syncwarp();
+    uint32_t n_heads = 0;
+    for (int s = 0; s < kApplyTile / 32; ++s) {
+      const int o = 32 * s + lane;
+      const unsigned long long e = base + o;
+      const uint32_t key = s_key[wb][o];
+      bool head = key != kSkipRecord && (o > 0 ? s_key[wb][o - 1] != key : (e == 0 || keys[e - 1] != key));
+      if (head && e + kShortRun < total) {
+        // a run longer than kShortRun belongs to a warp of the first phase
+        head = (o + kShortRun < kApplyTile ? s_key[wb][o + kShortRun] : keys[e + kShortRun]) != key;
+      }
+      const unsigned m = __ballot_sync(0xffffffffu, head);
+      if (head) s_head[wb][n_heads + __popc(m & ((1u << lane) - 1u))] = (uint8_t)o;
+      n_heads += __popc(m);
+    }
+    __syncwarp();
+    for (uint32_t h = lane; h < n_heads; h += 32) {
+      const int o = s_head[wb][h];
+      const uint32_t key = s_key[wb][o];
+      const VoxelRef vr = locate_voxel(P, tab, key);
+      if (vr.ptr == nullptr) continue;
+      TsdfVoxel v = *vr.ptr;
+      int k = o;
+      for (; k < kApplyTile && s_key[wb][k] == key; ++k) apply_update(v, s_sdf[wb][k], s_w[wb][k], s_col[wb][k], P.up);
+      if (k == kApplyTile) {
+        // a run that crosses the tile's end continues from global memory
+        for (unsigned long long j = base + kApplyTile; j < total && keys[j] == key; ++j) {
+          apply_update(v, rec_sdf[j], rec_w[j], rec_col[j], P.up);
+        }
+      }
+      *vr.ptr = v;
+    }
+    __syncwarp();  // the staging arrays are reused by the warp's next tile
   }
 }
 
@@ -2120,28 +2170,24 @@ static int sort_and_apply(vbx_ctx* c, const ScanParams& P, unsigned long long K,
     rv.d_total = &c->d_state->total_updates;
     rv.total_fixed = 0;
   }
+  LongRuns lr;
+  lr.start = c->long_list;
+  lr.end = c->long_end;
+  lr.keep = c->keep_bits;
+  lr.cap = c->max_updates / 32 + 1;
+  // everything of the apply that does not depend on the map, on the (pipelined: scan-private) sort stream
+  k_apply_prep<<<c->grid_sms * 8, 256, 0, s>>>(P, c->tab, rv, c->ray_a, c->ray_c, lr, c->d_state);
   mk.mark(6);
   if (c->apply_stream) {
-    // pipelined submission: the apply kernels run on their own stream behind the sort, so the
+    // pipelined submission: the apply kernel runs on its own stream behind the sort, so the
     // next scan's ray walk can start while this scan's voxels are still being written
     VBX_CUDA(c, cudaEventRecord(c->sorted_event, s));
     VBX_CUDA(c, cudaStreamWaitEvent(c->apply_stream, c->sorted_event, 0));
     s = c->apply_stream;
   }
-  const unsigned int g_short = c->grid_sms * 8;
-  LongRuns lr;
-  lr.start = c->long_list;
-  lr.end = c->long_end;
-  lr.state = c->long_state;
-  lr.item_run = c->verify_run;
-  lr.item_start = c->verify_start;
-  lr.rec_sdf = c->rec_sdf;
-  lr.rec_w = c->rec_w;
-  k_apply_short<<<g_short, 256, 0, s>>>(P, c->tab, rv, c->ray_a, c->ray_c, lr, c->d_state);
-  k_apply_verify<<<c->grid_sms * 8, 128, 0, s>>>(P, c->tab, rv, c->ray_a, c->ray_c, lr, c->d_state);
-  k_apply_long<<<c->grid_sms * 4, 128, 0, s>>>(P, c->tab, rv, c->ray_a, c->ray_c, lr, c->d_state);
+  k_apply<<<c->grid_sms * 8, 32 * kApplyWarps, 0, s>>>(P, c->tab, rv, lr, c->d_state);
   mk.mark(7);
-  *launches += 3;
+  *launches += 2;
   return VBX_OK;
 }
 
