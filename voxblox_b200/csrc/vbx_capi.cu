@@ -135,6 +135,8 @@ void select_set(vbx_ctx* c, int k) {
   c->off = S.off;
   c->d_state = S.d_state;
   c->h_state = S.h_state;
+  c->d_args = S.d_args;
+  c->h_args = S.h_args;
   c->d_xyz = S.d_xyz;
   c->d_rgba = S.d_rgba;
   c->pkeys[0] = S.pkeys0;
@@ -176,8 +178,6 @@ int drain_async(vbx_ctx* c) {
   select_set(c, 0);
   select_lane(c, 0);
   c->stream = c->stream_main;
-  c->apply_stream = nullptr;
-  c->sort_stream = nullptr;
   if (int rc = recover_async(c)) {
     if (!c->deferred_rc) return rc;
   }
@@ -411,6 +411,9 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
     a.off = c->off;
     a.d_state = c->d_state;
     a.h_state = c->h_state;
+    if (int rc = alloc_scan_args(c, a)) return rc;
+    c->d_args = a.d_args;
+    c->h_args = a.h_args;
     a.d_xyz = c->d_xyz;
     a.d_rgba = c->d_rgba;
     a.pkeys0 = c->pkeys[0];
@@ -454,14 +457,13 @@ int ensure_async(vbx_ctx* c) {
   if (const char* e = std::getenv("VBX_ASYNC_SETS")) c->sets_in_use = std::max(2, std::min(std::atoi(e), (int)vbx_ctx::kSets));
   if (const char* e = std::getenv("VBX_ASYNC_LANES")) c->lanes_in_use = std::max(1, std::min(std::atoi(e), (int)vbx_ctx::kLanes));
   const size_t np = c->max_points;
-  CK(cudaStreamCreateWithFlags(&c->stream_h, cudaStreamNonBlocking));
   CK(cudaStreamCreateWithPriority(&c->stream_e, cudaStreamNonBlocking, std::min(c->prio_lo, c->prio_hi + 1)));
-  for (int i = 0; i < vbx_ctx::kSortStreams; ++i) {
-    CK(cudaStreamCreateWithPriority(&c->stream_s[i], cudaStreamNonBlocking, std::min(c->prio_lo, c->prio_hi + 2)));
-  }
+  CK(cudaStreamCreateWithPriority(&c->stream_s, cudaStreamNonBlocking, std::min(c->prio_lo, c->prio_hi + 2)));
+  for (cudaEvent_t& e : c->cap_ev) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   for (int l = 0; l < c->lanes_in_use; ++l) {
     vbx_ctx::FrontLane& F = c->lane[l];
     CK(cudaStreamCreateWithPriority(&F.stream, cudaStreamNonBlocking, c->prio_lo));
+    CK(cudaEventCreateWithFlags(&F.done, cudaEventDisableTiming));
     if (l == 0) continue;
     CK(dmalloc(&F.pkeys1, np));
     CK(dmalloc(&F.pvals[0], np));
@@ -480,14 +482,18 @@ int ensure_async(vbx_ctx* c) {
   }
   for (int k = 0; k < c->sets_in_use; ++k) {
     vbx_ctx::ScratchSet& S = c->set[k];
+    CK(cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking));
     CK(cudaEventCreateWithFlags(&S.copy_done, evf));
-    CK(cudaEventCreateWithFlags(&S.front_done, evf));
     CK(cudaEventCreateWithFlags(&S.walked, evf));
     CK(cudaEventCreateWithFlags(&S.sorted, evf));
     CK(cudaEventCreateWithFlags(&S.back_done, evf));
     CK(cudaEventCreateWithFlags(&S.applied, evf));
-    if (c->timeline) CK(cudaEventCreate(&S.front_start));
+    if (c->timeline) {
+      CK(cudaEventCreate(&S.front_start));
+      CK(cudaEventCreate(&S.front_done));
+    }
     if (k == 0) continue;
+    if (int rc = alloc_scan_args(c, S)) return rc;
     CK(dmalloc(&S.ray_p, np));
     CK(dmalloc(&S.ray_a, np));
     CK(dmalloc(&S.ray_c, np));
@@ -525,10 +531,8 @@ void vbx_destroy(vbx_ctx* c) {
   if (c->stream_main) cudaStreamSynchronize(c->stream_main);
   if (c->stream_c) cudaStreamSynchronize(c->stream_c);
   if (c->stream_c2) cudaStreamSynchronize(c->stream_c2);
-  if (c->stream_h) cudaStreamSynchronize(c->stream_h);
-  if (c->stream_e) cudaStreamSynchronize(c->stream_e);
-  for (int i = 0; i < vbx_ctx::kSortStreams; ++i) {
-    if (c->stream_s[i]) cudaStreamSynchronize(c->stream_s[i]);
+  for (int k = 0; k < vbx_ctx::kSets; ++k) {
+    if (c->set[k].stream) cudaStreamSynchronize(c->set[k].stream);
   }
   for (int l = 0; l < vbx_ctx::kLanes; ++l) {
     if (c->lane[l].stream) cudaStreamSynchronize(c->lane[l].stream);
@@ -567,6 +571,15 @@ void vbx_destroy(vbx_ctx* c) {
       }
       if (S.h_state) cudaFreeHost(S.h_state);
     }
+    if (S.d_args) cudaFree(S.d_args);
+    if (S.h_args) cudaFreeHost(S.h_args);
+    for (auto& per_lane : S.graph) {
+      for (vbx_ctx::ScanGraph& G : per_lane) {
+        if (G.exec) cudaGraphExecDestroy(G.exec);
+        if (G.graph) cudaGraphDestroy(G.graph);
+      }
+    }
+    if (S.stream) cudaStreamDestroy(S.stream);
     if (S.copy_done) cudaEventDestroy(S.copy_done);
     if (S.front_done) cudaEventDestroy(S.front_done);
     if (S.walked) cudaEventDestroy(S.walked);
@@ -590,6 +603,7 @@ void vbx_destroy(vbx_ctx* c) {
     }
     if (F.ev_fork) cudaEventDestroy(F.ev_fork);
     if (F.ev_join) cudaEventDestroy(F.ev_join);
+    if (F.done) cudaEventDestroy(F.done);
     if (F.stream) cudaStreamDestroy(F.stream);
   }
   if (c->timeline_ref) cudaEventDestroy(c->timeline_ref);
@@ -602,12 +616,12 @@ void vbx_destroy(vbx_ctx* c) {
   }
   if (c->stream_main) cudaStreamDestroy(c->stream_main);
   if (c->stream_e) cudaStreamDestroy(c->stream_e);
-  for (int i = 0; i < vbx_ctx::kSortStreams; ++i) {
-    if (c->stream_s[i]) cudaStreamDestroy(c->stream_s[i]);
+  if (c->stream_s) cudaStreamDestroy(c->stream_s);
+  for (cudaEvent_t e : c->cap_ev) {
+    if (e) cudaEventDestroy(e);
   }
   if (c->stream_c) cudaStreamDestroy(c->stream_c);
   if (c->stream_c2) cudaStreamDestroy(c->stream_c2);
-  if (c->stream_h) cudaStreamDestroy(c->stream_h);
   delete c;
 }
 

@@ -16,6 +16,7 @@
 
 namespace vbx {
 struct SortPlan;
+struct ScanArgs;  // a scan's per-call kernel arguments in device memory (vbx_tsdf.cu)
 }
 
 namespace vbx {
@@ -145,7 +146,6 @@ struct vbx_ctx {
   cudaStream_t stream_main = nullptr; // back halves, ESDF, block management, synchronous calls
   cudaStream_t stream_c = nullptr;    // host-to-device cloud copies of asynchronously submitted scans
   cudaStream_t stream_c2 = nullptr;   // ... alternating with this one
-  cudaStream_t stream_h = nullptr;    // read-back of a queued scan's status block (keeps the copy engine out of the apply stream)
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   vbx_tsdf_config cfg;
   vbx_engine_options opt;
@@ -198,18 +198,33 @@ struct vbx_ctx {
   int64_t fast_reset_counter = 0;
   vbx::ScanState* d_state = nullptr;
   vbx::ScanState* h_state = nullptr;  // pinned
+  vbx::ScanArgs* d_args = nullptr;    // the current hand-off set's argument block ...
+  vbx::ScanArgs* h_args = nullptr;    // ... and its page-locked host copy
   uint32_t epoch = 0;                 // call id for touch marks
   uint32_t n_blocks = 0;              // pool slots in use (host copy, exact after a drain)
   uint32_t* d_nblocks = nullptr;      // [2] device copy, ping-pong: k_assign reads [nb_cur], writes [nb_cur ^ 1]
   int nb_cur = 0;
-  // Asynchronous submission (vbx_tsdf_integrate_async): a scan passes through three stages on
-  // separate streams -- front half (keys, bundle sort, bundle fold, offsets; does not touch the map)
-  // on one of kLanes front streams, ray walk + block creation + record sort on stream_e, apply on
-  // the main stream -- so up to kSets scans are in flight, each owning one set of hand-off
-  // buffers.  Map-touching stages run in submission order.  Set 0 / lane 0 are the buffers the
-  // synchronous calls use; the others are allocated on the first asynchronous submission.
-  static constexpr int kSets = 16, kLanes = 8, kSortStreams = 2;  // upper bounds
+  // Asynchronous submission (vbx_tsdf_integrate_async): a scan passes through four stages -- front half
+  // (keys, bundle sort, bundle fold, offsets; does not touch the map) on one of kLanes front lanes, ray
+  // walk + block creation, record sort, apply -- so up to kSets scans are in flight, each owning one set
+  // of hand-off buffers.  Map-touching stages run in submission order.  Each scan is one launch of a CUDA
+  // graph per (hand-off set, front lane, kind), captured before its first use.  Set 0 / lane 0 are the
+  // buffers the synchronous calls use; the others are allocated on the first asynchronous submission.
+  static constexpr int kSets = 16, kLanes = 8;  // upper bounds
   int sets_in_use = 10, lanes_in_use = 6;  // (tuning aids: VBX_ASYNC_SETS, VBX_ASYNC_LANES)
+  enum { kGraphSimple, kGraphMerged, kGraphVariants };
+  struct ScanGraph {
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    uint64_t launches = 0;                  // kernel nodes
+    cudaGraphNode_t point_sort = nullptr;   // grid sized by the scan's point count
+    unsigned int point_grid = 0;
+    cudaGraphNode_t record_sort = nullptr;  // grid sized by record_hint
+    unsigned int record_grid = 0;
+    cudaGraphNode_t order = nullptr;        // k_bundle_order: form and shared memory follow bundle_hint
+    unsigned int order_grid = 0;
+    size_t order_smem = 0;
+  };
   struct ScratchSet {
     float4* ray_p = nullptr;
     float4* ray_a = nullptr;
@@ -221,6 +236,8 @@ struct vbx_ctx {
     uint32_t* off = nullptr;
     vbx::ScanState* d_state = nullptr;
     vbx::ScanState* h_state = nullptr;
+    vbx::ScanArgs* d_args = nullptr;
+    vbx::ScanArgs* h_args = nullptr;  // page-locked: the graph's first node uploads it
     float* d_xyz = nullptr;
     uint8_t* d_rgba = nullptr;
     uint64_t* pkeys0 = nullptr;  // sorted bundle keys (read again by the ray walk)
@@ -231,9 +248,10 @@ struct vbx_ctx {
     uint32_t* keep_bits = nullptr;
     vbx::SortPlan* sort_plan1 = nullptr;
     uint32_t* sort_status1 = nullptr;
-    cudaEvent_t copy_done = nullptr, front_done = nullptr, walked = nullptr, sorted = nullptr, back_done = nullptr;
-    cudaEvent_t applied = nullptr;      // the apply kernels are done (the status read-back follows on stream_h)
-    cudaEvent_t front_start = nullptr;  // only with VBX_ASYNC_TIMELINE (vbx_debug_async_timeline)
+    cudaEvent_t copy_done = nullptr, walked = nullptr, sorted = nullptr, applied = nullptr, back_done = nullptr;
+    cudaEvent_t front_start = nullptr, front_done = nullptr;  // only with VBX_ASYNC_TIMELINE (vbx_debug_async_timeline)
+    cudaStream_t stream = nullptr;  // the scan's graph is launched here (one stream per set: graphs in one stream run one after the other)
+    ScanGraph graph[kLanes][kGraphVariants];
     bool in_flight = false;
     int kind = 0;
     uint64_t launches = 0;
@@ -259,15 +277,22 @@ struct vbx_ctx {
     vbx::OrderScratch order_scratch{};
     cudaStream_t side = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+    cudaEvent_t done = nullptr;  // the lane's last front half
   } lane[kLanes];
   bool async_ready = false;
   int prio_lo = 0, prio_hi = 0;  // stream priority range of the device
-  cudaStream_t stream_e = nullptr;      // ray walk + block creation + record sort of asynchronously submitted scans
-  cudaStream_t stream_s[kSortStreams] = {nullptr, nullptr};  // record sorts (set-private buffers: independent across scans)
-  cudaStream_t sort_stream = nullptr;   // non-null while an asynchronous back half is enqueued: the record sort goes here
-  cudaEvent_t walked_event = nullptr;   // ... after this event
-  cudaStream_t apply_stream = nullptr;  // ... and the apply kernels here
-  cudaEvent_t sorted_event = nullptr;   // ... after this event
+  // the streams a scan's graph is captured from (besides the front lane's and the main stream)
+  cudaStream_t stream_e = nullptr;  // ray walk + block creation
+  cudaStream_t stream_s = nullptr;  // record sort + apply preparation
+  // non-null while a scan's graph is captured: the back half's streams and hand-off events (integrate_async)
+  struct Capture {
+    cudaStream_t sort, apply;
+    cudaEvent_t walked, sorted, applied;   // this scan's stage ends: later scans' graphs wait for them
+    cudaEvent_t prev_sorted, prev_applied; // the record sort two scans back, the previous scan's apply
+    cudaEvent_t edge[2];                   // capture-internal: walk -> sort, sort -> apply
+  };
+  const Capture* cap = nullptr;
+  cudaEvent_t cap_ev[8] = {};  // capture-internal edges (fork, front -> walk, walk -> sort, sort -> apply, joins)
   uint64_t async_seq = 0;
   uint32_t* d_hold = nullptr;           // device flag: a queued scan must be redone, later scans skip their back half
   uint64_t async_redone = 0;            // scans redone synchronously since vbx_create (reporting)
@@ -362,6 +387,7 @@ void free_order_scratch(vbx::OrderScratch* g, uint32_t* big_list, uint32_t* firs
 int init_bundle_order(vbx_ctx* c);     // rehash schedule + shared-memory opt-in of k_bundle_order
 int rebuild_hash(vbx_ctx* c);          // block hash rebuilt from slot_key (after removals / a pool overflow)
 void harvest_async(vbx_ctx* c, vbx_ctx::ScratchSet& S);  // collect a finished asynchronous scan's results
+int alloc_scan_args(vbx_ctx* c, vbx_ctx::ScratchSet& S);  // the set's argument block, device + page-locked host
 }  // namespace vbx
 
 #define VBX_CUDA(c, expr)                                          \

@@ -329,7 +329,7 @@ k_sort(KeyT* keys_a, uint32_t* vals_a, KeyT* keys_b, uint32_t* vals_b, const uns
   }
 }
 
-// Exclusive prefix sum of n uint32 (n known on the host), chained scan over tiles of 2048.  With a
+// Exclusive prefix sum of n uint32 (n = *d_n, or n_fixed), chained scan over tiles of 2048.  With a
 // permutation the summand at position i is in[perm[i]] for i < *d_limit and 0 beyond (the record
 // offsets of the Merged integrator: counts are stored per bundle id, offsets are needed in rank order;
 // a few thousand bundles out of a launch sized for every point its own bundle).
@@ -337,9 +337,10 @@ constexpr int kScanItems = 8;
 constexpr int kScanTile = kSortThreads * kScanItems;
 static __global__ void __launch_bounds__(kSortThreads)
 k_exclusive_scan(const uint32_t* __restrict__ in, const uint32_t* __restrict__ perm, const uint32_t* __restrict__ d_limit,
-                 uint32_t* __restrict__ out, uint32_t n, uint32_t* status, uint32_t* tile_counter,
-                 unsigned long long* total_out, unsigned long long* total_ok_out, uint32_t* error_word,
-                 unsigned long long total_max, uint32_t error_bit) {
+                 uint32_t* __restrict__ out, const uint32_t* __restrict__ d_n, uint32_t n_fixed, uint32_t* status,
+                 uint32_t* tile_counter, unsigned long long* total_out, unsigned long long* total_ok_out,
+                 uint32_t* error_word, unsigned long long total_max, uint32_t error_bit) {
+  const uint32_t n = d_n ? *d_n : n_fixed;
   const uint32_t limit = d_limit ? *d_limit : 0xffffffffu;
   // with a limit only positions [0, limit] are scanned (position `limit` holds the total: its summand is 0);
   // the total is also stored at out[n - 1], where the callers read it -- positions in between are not written

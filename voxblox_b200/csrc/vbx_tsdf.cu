@@ -36,6 +36,7 @@
 #include <chrono>
 #include <cstdio>
 #include <cstring>
+#include <numeric>
 #include <unordered_map>  // std::__detail::_Prime_rehash_policy: the growth schedule the reference's map follows
 
 #include <cooperative_groups.h>
@@ -78,6 +79,17 @@ struct ScanParams {
   // a call whose update records do not fit max_updates_per_pass is emitted and applied in several
   // passes over contiguous ray-slot ranges [emit_lo, emit_hi); emit_base = off[emit_lo]
   uint32_t emit_lo, emit_hi, emit_base;
+};
+
+// Everything a scan's kernels take that changes from scan to scan, in device memory (one block per hand-off
+// set, ScratchSet::d_args): the kernel nodes of a scan's CUDA graph are built once and read it at run time.
+struct ScanArgs {
+  ScanParams P;
+  const float* xyz;
+  const uint8_t* rgba;
+  unsigned long long n;  // P.n: the point sort's element count
+  uint32_t n_scan;       // P.n + 1: positions of the record-offset scan
+  uint32_t nb_cur;       // k_assign reads d_nblocks[nb_cur], writes d_nblocks[nb_cur ^ 1]
 };
 
 // MixedThreadSafeIndex::getNextIndexImpl, integrator_utils.cc:54-63
@@ -160,8 +172,10 @@ __device__ __forceinline__ I3 key_voxel(const KeyLayout& k, uint64_t key) {
 // Merged, pass 1 over the cloud: the bounding box of the valid points' voxels (and their count).
 // Grid-stride over the points, one set of atomics per thread block.
 __global__ void __launch_bounds__(256)
-k_point_bounds(ScanParams P, const float* __restrict__ xyz, uint32_t* __restrict__ first_bits, SortPlan* plan,
+k_point_bounds(const ScanArgs* __restrict__ A, uint32_t* __restrict__ first_bits, SortPlan* plan,
                uint32_t* __restrict__ scan_status, uint32_t scan_words, ScanState* st) {
+  const ScanParams P = A->P;
+  const float* __restrict__ xyz = A->xyz;
   __shared__ uint32_t s_red[7];
   if (threadIdx.x < 7) s_red[threadIdx.x] = 0u;
   const uint32_t words2 = 2u * ((P.n + 31u) >> 5);
@@ -219,8 +233,10 @@ k_point_bounds(ScanParams P, const float* __restrict__ xyz, uint32_t* __restrict
 // Merged, pass 2: key every point by its end voxel (bundleRays, cc:340-371), in the reference's
 // point order (position s of that order holds point point_order(s)).
 template <typename KeyT>
-__global__ void k_point_keys(ScanParams P, const float* __restrict__ xyz, const uint32_t* __restrict__ order,
+__global__ void k_point_keys(const ScanArgs* __restrict__ A, const uint32_t* __restrict__ order,
                              KeyT* __restrict__ keys, uint32_t* __restrict__ vals, ScanState* st) {
+  const ScanParams P = A->P;
+  const float* __restrict__ xyz = A->xyz;
   const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
   const KeyLayout kl = key_layout(st);
   if (s == 0) st->key_bits = (uint32_t)(kl.bx + kl.by + kl.bz + 1);
@@ -274,10 +290,11 @@ constexpr uint32_t kHeadBig = 0x80000000u;   // head_list entry: sorted position
 // voxel_map / clear_map (bundleRays, cc:340-371).  k_bundle_order turns them into the maps'
 // iteration order.
 template <typename KeyT>
-__global__ void k_heads(ScanParams P, const KeyT* __restrict__ keys, const uint32_t* __restrict__ vals,
+__global__ void k_heads(const ScanArgs* __restrict__ A, const KeyT* __restrict__ keys, const uint32_t* __restrict__ vals,
                         const uint32_t* __restrict__ order_inv, uint32_t* __restrict__ head_list,
                         uint32_t* __restrict__ big_list, uint32_t* __restrict__ first_bits, uint32_t* __restrict__ cnt,
                         ScanState* st) {
+  const ScanParams P = A->P;
   const uint32_t n = P.n;
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   const KeyLayout kl = key_layout(st);
@@ -328,7 +345,8 @@ __device__ __forceinline__ uint32_t long_index_hash(int x, int y, int z) {
 //                   (cooperative launch), the early (small) stages still in block 0's shared memory.
 // The clearing map's arrays follow the normal map's at offset g.cap.
 __global__ void __launch_bounds__(kOrderThreads)
-k_order_prefix(uint32_t n, const uint32_t* __restrict__ first_bits, OrderScratch g, ScanState* st) {
+k_order_prefix(const ScanArgs* __restrict__ A, const uint32_t* __restrict__ first_bits, OrderScratch g, ScanState* st) {
+  const uint32_t n = A->P.n;
   __shared__ uint32_t warp_sums[33];
   const uint32_t tid = threadIdx.x;
   const uint32_t words = (n + 31u) >> 5;
@@ -352,9 +370,10 @@ k_order_prefix(uint32_t n, const uint32_t* __restrict__ first_bits, OrderScratch
 }
 
 template <typename KeyT>
-__global__ void k_order_heads(ScanParams P, const KeyT* __restrict__ keys, const uint32_t* __restrict__ vals,
+__global__ void k_order_heads(const ScanArgs* __restrict__ A, const KeyT* __restrict__ keys, const uint32_t* __restrict__ vals,
                               const uint32_t* __restrict__ order_inv, const uint32_t* __restrict__ head_list,
                               const uint32_t* __restrict__ first_bits, OrderScratch g, const ScanState* st) {
+  const ScanParams P = A->P;
   const uint32_t words = (P.n + 31u) >> 5;
   const uint32_t n_heads = st->n_ray_list;
   const KeyLayout kl = key_layout(st);
@@ -795,11 +814,14 @@ __device__ __forceinline__ void consumer_barrier(int triple_in_block) {
 // instructions (~5 dependent operations per member for the mean, ~7 for a colour channel).
 template <typename KeyT>
 __global__ void __launch_bounds__(192)
-k_merge(ScanParams P, const float* __restrict__ xyz, const uint8_t* __restrict__ rgba,
+k_merge(const ScanArgs* __restrict__ A,
         const KeyT* __restrict__ keys, const uint32_t* __restrict__ vals, const uint32_t* __restrict__ head_list,
         const uint32_t* __restrict__ big_list,
         float4* __restrict__ ray_p, float4* __restrict__ ray_a, uint2* __restrict__ ray_c, uint32_t* __restrict__ cnt,
         ScanState* st) {
+  const ScanParams P = A->P;
+  const float* __restrict__ xyz = A->xyz;
+  const uint8_t* __restrict__ rgba = A->rgba;
   __shared__ float4 stage[2][2][32 * kStageStride];  // [pair in block][slot][member][role]
   __shared__ ChunkDesc desc[2][2];
   const int lane = threadIdx.x & 31;
@@ -1093,12 +1115,14 @@ __device__ __forceinline__ bool replace_hash(unsigned long long* set, uint32_t h
 // dense ray list; Simple / Fast build their ray from point slot i (integrateFunction,
 // cc:269-305 / :488-553).
 template <typename KeyT>
-__global__ void k_rays_count(ScanParams P, Tables tab, const float* __restrict__ xyz,
-                             const uint8_t* __restrict__ rgba, const uint32_t* __restrict__ order,
+__global__ void k_rays_count(const ScanArgs* __restrict__ A, Tables tab, const uint32_t* __restrict__ order,
                              const KeyT* __restrict__ keys, const uint32_t* __restrict__ head_list,
                              float4* __restrict__ ray_p, float4* __restrict__ ray_a, uint2* __restrict__ ray_c,
                              uint32_t* __restrict__ cnt,
                              unsigned long long* set_start, unsigned long long* set_observed, ScanState* st) {
+  const ScanParams P = A->P;
+  const float* __restrict__ xyz = A->xyz;
+  const uint8_t* __restrict__ rgba = A->rgba;
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   uint32_t i;
   F3 point_G;
@@ -1205,8 +1229,10 @@ __global__ void k_back_begin(ScanState* st, uint32_t* hold) {
 
 // After the last walk that can create blocks: pool slots for the blocks created by this call
 // (updateLayerWithStoredBlocks, cc:137-147); a new block is born with all updated bits set (cc:128).
-__global__ void k_assign(Tables tab, const uint32_t* __restrict__ nb_in, uint32_t* __restrict__ nb_out, SortPlan* record_plan,
+__global__ void k_assign(Tables tab, const ScanArgs* __restrict__ A, uint32_t* __restrict__ nb, SortPlan* record_plan,
                          ScanState* st) {
+  const uint32_t* __restrict__ nb_in = nb + A->nb_cur;
+  uint32_t* __restrict__ nb_out = nb + (A->nb_cur ^ 1u);
   const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j < (uint32_t)(sizeof(SortPlan) / 4)) reinterpret_cast<uint32_t*>(record_plan)[j] = 0u;  // for the record sort that follows
   const uint32_t n_blocks_before = *nb_in;
@@ -1298,11 +1324,12 @@ __device__ void emit_ray_sequential(const ScanParams& P, const Tables& tab, cons
 }
 
 template <typename KeyT>
-__global__ void k_rays_emit(ScanParams P, Tables tab, const KeyT* __restrict__ keys,
+__global__ void k_rays_emit(const ScanArgs* __restrict__ A, Tables tab, const KeyT* __restrict__ keys,
                             const uint32_t* __restrict__ ray_list, const uint32_t* __restrict__ head_list,
                             const float4* __restrict__ ray_p, const uint32_t* __restrict__ cnt,
                             const uint32_t* __restrict__ off, uint32_t* __restrict__ ckeys,
                             uint32_t* __restrict__ cvals, ScanState* st) {
+  const ScanParams P = A->P;
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   uint32_t i;
   uint32_t head_pos = 0;
@@ -1335,9 +1362,10 @@ constexpr int kWalkCap = 3 * kChainCap;
 
 template <typename KeyT>
 __global__ void __launch_bounds__(128)
-k_rays_emit_warp(ScanParams P, Tables tab, const KeyT* __restrict__ keys, const uint32_t* __restrict__ ray_list,
+k_rays_emit_warp(const ScanArgs* __restrict__ A, Tables tab, const KeyT* __restrict__ keys, const uint32_t* __restrict__ ray_list,
                  const uint32_t* __restrict__ head_list, const float4* __restrict__ ray_p, const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ off,
                  uint32_t* __restrict__ ckeys, uint32_t* __restrict__ cvals, ScanState* st) {
+  const ScanParams P = A->P;
   __shared__ float chain_s[4][3][kChainCap];
   __shared__ uint32_t walk_s[4][kWalkCap];
   const int lane = threadIdx.x & 31;
@@ -1545,8 +1573,9 @@ __device__ __forceinline__ Prepared open_prepared(const RecordView& rv) {
 // runs longer than kShortRun updates with their [start, end).  Records of blocks this rank does not
 // own (kSkipRecord) sort to the end and are skipped.
 __global__ void __launch_bounds__(256, 6)
-k_apply_prep(ScanParams P, Tables tab, RecordView rv, const float4* __restrict__ ray_a,
+k_apply_prep(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, const float4* __restrict__ ray_a,
              const uint2* __restrict__ ray_c, LongRuns lr, ScanState* st) {
+  const ScanParams P = A->P;
   const uint32_t sel = rv.plan ? rv.plan->final_buf : 0u;
   const uint32_t* __restrict__ keys = rv.keys[sel];
   uint32_t* __restrict__ vals = rv.vals[sel];
@@ -1650,7 +1679,8 @@ __device__ __forceinline__ unsigned long long keep_suffix(const uint32_t* __rest
 // distance chain.  Once the voxel rests at (+T, max_weight) and every remaining record's keep bit is
 // set, the rest of the run leaves it unchanged and is skipped.
 __global__ void __launch_bounds__(32 * kApplyWarps, 8)
-k_apply(ScanParams P, Tables tab, RecordView rv, LongRuns lr, ScanState* st) {
+k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, ScanState* st) {
+  const ScanParams P = A->P;
   const Prepared pr = open_prepared(rv);
   if (st->error & kFatalErrors) return;
   const uint32_t* __restrict__ keys = pr.key;
@@ -2002,6 +2032,11 @@ struct Marks {
 };
 }  // namespace
 
+static unsigned int sort_grid(const vbx_ctx* c, int which, uint64_t n_hint) {
+  const uint64_t tiles_hint = std::max<uint64_t>(1, (n_hint + kSortTile - 1) / kSortTile);
+  return (unsigned int)std::min<uint64_t>(std::min<uint64_t>(c->sort_tiles_cap[which], tiles_hint), (uint64_t)c->grid_sms * 2);
+}
+
 // The engine's own stable radix sort (vbx_sort.cuh): one launch.  n lives on the device (d_n) or is n_fixed;
 // n_hint sizes the grid (tiles are handed out by ticket, so any grid sorts any n).  result_in_a: the sorted
 // pairs end in buffer A whatever the number of passes (otherwise SortPlan::final_buf says where they are).
@@ -2015,8 +2050,7 @@ static int own_sort(vbx_ctx* c, int which, KeyT* keys_a, uint32_t* vals_a, KeyT*
   uint32_t* status = c->sort_status[which];
   const uint32_t tiles_cap = c->sort_tiles_cap[which];
   if (!plan_cleared) VBX_CUDA(c, cudaMemsetAsync(plan, 0, sizeof(SortPlan), s));  // (else: an earlier kernel of the stream did)
-  const uint64_t tiles_hint = std::max<uint64_t>(1, (n_hint + kSortTile - 1) / kSortTile);
-  const unsigned int grid = (unsigned int)std::min<uint64_t>(std::min<uint64_t>(tiles_cap, tiles_hint), (uint64_t)c->grid_sms * 2);
+  const unsigned int grid = sort_grid(c, which, n_hint);
   k_sort<KeyT><<<grid, kSortThreads, 0, s>>>(keys_a, vals_a, keys_b, vals_b, d_n, n_fixed, passes, d_key_bits, plan, status,
                                               tiles_cap, result_in_a ? 1 : 0);
   *launches += 1;
@@ -2029,68 +2063,85 @@ constexpr int kOrderGrid = 32;  // blocks of the cooperative k_bundle_order laun
 // SM: a block that wants 200 KB can only start on an SM that holds nothing else, and in the pipelined path
 // -- every SM busy with other scans' kernels -- it waits for one to drain.  A scan with more bundles than the
 // request covers is still ordered correctly: the kernel falls back to its global-memory stages.
-template <typename KeyT>
-static int launch_bundle_order(vbx_ctx* c, cudaStream_t so, const ScanParams& P, const KeyT* keys, const uint32_t* vals) {
-  k_order_prefix<<<1, kOrderThreads, 0, so>>>(P.n, c->first_bits, c->order_scratch, c->d_state);
-  k_order_heads<KeyT><<<std::min<unsigned int>(grid_for(P.n, 256), c->grid_sms * 2), 256, 0, so>>>(
-      P, keys, vals, c->order_inv, c->head_list, c->first_bits, c->order_scratch, c->d_state);
-  RehashSchedule rs = c->rehash;
-  size_t smem_bytes = c->order_smem_bytes;
-  unsigned int grid = kOrderGrid;
+struct OrderLaunch {
+  unsigned int grid;  // 1: the one-block form, else the cooperative one
+  size_t smem_bytes;
+};
+static OrderLaunch order_launch(const vbx_ctx* c, uint32_t n) {
+  OrderLaunch o{(unsigned int)kOrderGrid, c->order_smem_bytes};
   if (c->bundle_hint) {
-    const uint32_t B = (uint32_t)std::min<uint64_t>(c->bundle_hint + c->bundle_hint / 4 + 512, P.n);
+    const RehashSchedule& rs = c->rehash;
+    const uint32_t B = (uint32_t)std::min<uint64_t>(c->bundle_hint + c->bundle_hint / 4 + 512, n);
     uint32_t nf = 1;
     for (int k = 0; k < rs.count && rs.m[k] < B; ++k) nf = rs.n[k];
     const uint32_t words = order_smem_words_needed(B, nf);
     const size_t need = ((size_t)words * 4 + 1023) & ~(size_t)1023;
     if (words != 0xffffffffu && need <= c->order_smem_bytes) {
-      smem_bytes = need;
-      grid = 1;  // the single-block form; block 0 is the only one that would work
+      o.smem_bytes = need;
+      o.grid = 1;  // the single-block form; block 0 is the only one that would work
     }
   }
-  OrderScratch g = c->order_scratch;
-  uint32_t smem_words = (uint32_t)(smem_bytes / 4);
-  uint32_t* ray_list = c->ray_list;
-  uint32_t* cta_tot = c->order_scratch.cta_tot;
-  ScanState* st = c->d_state;
-  void* args[] = {&rs, &g, &smem_words, &ray_list, &cta_tot, &st};
-  if (grid == 1) {
-    // an ordinary launch: nothing about it has to be co-scheduled
-    k_bundle_order<<<1, kOrderThreads, smem_bytes, so>>>(rs, g, smem_words, ray_list, cta_tot, st);
-  } else {
-    VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_bundle_order, dim3(grid), dim3(kOrderThreads), args, smem_bytes, so));
-  }
+  return o;
+}
+
+template <typename KeyT>
+static int launch_bundle_order(vbx_ctx* c, cudaStream_t so, uint32_t n, const KeyT* keys, const uint32_t* vals) {
+  k_order_prefix<<<1, kOrderThreads, 0, so>>>(c->d_args, c->first_bits, c->order_scratch, c->d_state);
+  k_order_heads<KeyT><<<std::min<unsigned int>(grid_for(c->max_points, 256), c->grid_sms * 2), 256, 0, so>>>(
+      c->d_args, keys, vals, c->order_inv, c->head_list, c->first_bits, c->order_scratch, c->d_state);
+  // Always a cooperative launch (the one-block form is a cooperative grid of one block), so that a scan
+  // graph's node switches between the two forms by its grid and shared memory alone (update_scan_graph).
+  const OrderLaunch o = order_launch(c, n);
+  const uint32_t smem_words = (uint32_t)(o.smem_bytes / 4);
+  cudaLaunchConfig_t lc = {};
+  lc.gridDim = dim3(o.grid);
+  lc.blockDim = dim3(kOrderThreads);
+  lc.dynamicSmemBytes = o.smem_bytes;
+  lc.stream = so;
+  cudaLaunchAttribute coop;
+  coop.id = cudaLaunchAttributeCooperative;
+  coop.val.cooperative = 1;
+  lc.attrs = &coop;
+  lc.numAttrs = 1;
+  VBX_CUDA(c, cudaLaunchKernelEx(&lc, k_bundle_order, c->rehash, c->order_scratch, smem_words, c->ray_list,
+                                 c->order_scratch.cta_tot, c->d_state));
   return VBX_OK;
 }
 
-// Stages up to and including k_assign: everything that decides WHICH voxels are updated.
+// Stages up to and including k_assign: everything that decides WHICH voxels are updated.  The per-scan values
+// come from the argument block (c->d_args), and the grids are sized for max_points_per_scan -- surplus threads
+// exit at once -- so that one captured graph serves scans of any size (the point sort's grid, whose surplus
+// blocks would wait between passes, is set per scan instead: update_scan_graph).
 template <typename KeyT>
-static int front_half(vbx_ctx* c, ScanParams& P, const float* d_xyz, const uint8_t* d_rgba, const uint32_t* order,
-                      Marks& mk, uint64_t* launches, const KeyT** keys_out) {
+static int front_half(vbx_ctx* c, const ScanParams& P, const uint32_t* order, Marks& mk, uint64_t* launches,
+                      const KeyT** keys_out) {
   cudaStream_t s = c->stream;
+  const ScanArgs* A = c->d_args;
   const uint32_t n = P.n;
+  const uint32_t gn = c->max_points;
   const int TB = 256;
   const KeyT* keys = nullptr;
   const uint32_t* vals = nullptr;
   const uint32_t* scan_perm = nullptr;
   const uint32_t* scan_limit = nullptr;
+  const uint32_t scan_tiles = (gn + 1 + kScanTile - 1) / kScanTile;
   if (P.kind == VBX_MERGED) {
     KeyT* k0 = reinterpret_cast<KeyT*>(c->pkeys[0]);
     KeyT* k1 = reinterpret_cast<KeyT*>(c->pkeys[1]);
-    k_point_bounds<<<std::min<unsigned int>(grid_for(n, TB), c->grid_sms * 4), TB, 0, s>>>(
-        P, d_xyz, c->first_bits, c->sort_plan[0], c->scan_status, (n + 1 + kScanTile - 1) / kScanTile + 1, c->d_state);
-    k_point_keys<KeyT><<<grid_for(n, TB), TB, 0, s>>>(P, d_xyz, order, k0, c->pvals[0], c->d_state);
+    k_point_bounds<<<std::min<unsigned int>(grid_for(gn, TB), c->grid_sms * 4), TB, 0, s>>>(
+        A, c->first_bits, c->sort_plan[0], c->scan_status, scan_tiles + 1, c->d_state);
+    k_point_keys<KeyT><<<grid_for(gn, TB), TB, 0, s>>>(A, order, k0, c->pvals[0], c->d_state);
     mk.mark(0);
     // the bits in use are known on the device only (ScanState::key_bits): passes beyond them exit at once
-    if (int rc = own_sort<KeyT>(c, 0, k0, c->pvals[0], k1, c->pvals[1], nullptr, n, n, 8 * (int)sizeof(KeyT), true, launches,
-                                &c->d_state->key_bits, /*plan_cleared=*/true)) {
+    if (int rc = own_sort<KeyT>(c, 0, k0, c->pvals[0], k1, c->pvals[1], &A->n, 0, n, 8 * (int)sizeof(KeyT), true,
+                                launches, &c->d_state->key_bits, /*plan_cleared=*/true)) {
       return rc;
     }
     keys = k0;
     vals = c->pvals[0];
     mk.mark(1);
-    k_heads<KeyT><<<grid_for((uint64_t)n + 1, TB), TB, 0, s>>>(P, keys, vals, c->order_inv, c->head_list, c->big_list,
-                                                               c->first_bits, c->cnt, c->d_state);
+    k_heads<KeyT><<<grid_for((uint64_t)gn + 1, TB), TB, 0, s>>>(A, keys, vals, c->order_inv, c->head_list, c->big_list,
+                                                                c->first_bits, c->cnt, c->d_state);
     // The reference's bundle order (ray_list[rank] = bundle id, vbx_order.cuh) is one thread block's work
     // and the fold (k_merge) does not need it: the two run side by side.  (With stage profiling on they
     // run one after the other so that each gets its own time.)
@@ -2099,19 +2150,18 @@ static int front_half(vbx_ctx* c, ScanParams& P, const float* d_xyz, const uint8
       VBX_CUDA(c, cudaEventRecord(c->ev_fork, s));
       VBX_CUDA(c, cudaStreamWaitEvent(so, c->ev_fork, 0));
     }
-    if (int rc = launch_bundle_order<KeyT>(c, so, P, keys, vals)) return rc;
+    if (int rc = launch_bundle_order<KeyT>(c, so, P.n, keys, vals)) return rc;
     if (so != s) VBX_CUDA(c, cudaEventRecord(c->ev_join, so));
     mk.mark(12);
-    k_merge<KeyT><<<c->grid_sms * 4, 192, 0, s>>>(P, d_xyz, d_rgba, keys, vals, c->head_list, c->big_list, c->ray_p, c->ray_a,
-                                           c->ray_c, c->cnt, c->d_state);
+    k_merge<KeyT><<<c->grid_sms * 4, 192, 0, s>>>(A, keys, vals, c->head_list, c->big_list, c->ray_p, c->ray_a, c->ray_c,
+                                                  c->cnt, c->d_state);
     mk.mark(8);
     *launches += 8;
     if (!P.single_walk) {
       // the bundle count is only known on the device: launch for the worst case (every
       // point its own bundle); surplus threads exit on the first load
-      k_rays_count<KeyT><<<grid_for(n, 128), 128, 0, s>>>(P, c->tab, d_xyz, d_rgba, order, keys, c->head_list,
-                                                           c->ray_p, c->ray_a, c->ray_c, c->cnt, c->set_start,
-                                                           c->set_observed, c->d_state);
+      k_rays_count<KeyT><<<grid_for(gn, 128), 128, 0, s>>>(A, c->tab, order, keys, c->head_list, c->ray_p, c->ray_a,
+                                                           c->ray_c, c->cnt, c->set_start, c->set_observed, c->d_state);
       *launches += 1;
     }
     if (so != s) VBX_CUDA(c, cudaStreamWaitEvent(s, c->ev_join, 0));
@@ -2119,19 +2169,18 @@ static int front_half(vbx_ctx* c, ScanParams& P, const float* d_xyz, const uint8
     scan_perm = c->ray_list;
     scan_limit = &c->d_state->n_ray_list;
   } else {
-    k_rays_count<KeyT><<<grid_for((uint64_t)n + 1, 128), 128, 0, s>>>(P, c->tab, d_xyz, d_rgba, order, keys,
-                                                                       c->head_list, c->ray_p, c->ray_a, c->ray_c, c->cnt,
-                                                                       c->set_start, c->set_observed, c->d_state);
+    k_rays_count<KeyT><<<grid_for((uint64_t)gn + 1, 128), 128, 0, s>>>(A, c->tab, order, keys, c->head_list, c->ray_p,
+                                                                       c->ray_a, c->ray_c, c->cnt, c->set_start,
+                                                                       c->set_observed, c->d_state);
     *launches += 1;
   }
   mk.mark(2);
   {
     // record offsets; the scan's last position also settles the call's update count (total_found, total_updates,
     // kErrUpdatesFull: too many for one pass; nothing downstream runs on a call that failed)
-    const uint32_t tiles = (n + 1 + kScanTile - 1) / kScanTile;
-    if (P.kind != VBX_MERGED) VBX_CUDA(c, cudaMemsetAsync(c->scan_status, 0, (size_t)(tiles + 1) * sizeof(uint32_t), s));  // (Merged: k_point_bounds did)
-    k_exclusive_scan<<<std::min<uint32_t>(tiles, c->grid_sms * 4), kSortThreads, 0, s>>>(
-        c->cnt, scan_perm, scan_limit, c->off, n + 1, c->scan_status + 1, c->scan_status, &c->d_state->total_found,
+    if (P.kind != VBX_MERGED) VBX_CUDA(c, cudaMemsetAsync(c->scan_status, 0, (size_t)(scan_tiles + 1) * sizeof(uint32_t), s));  // (Merged: k_point_bounds did)
+    k_exclusive_scan<<<std::min<uint32_t>(scan_tiles, c->grid_sms * 4), kSortThreads, 0, s>>>(
+        c->cnt, scan_perm, scan_limit, c->off, &A->n_scan, 0u, c->scan_status + 1, c->scan_status, &c->d_state->total_found,
         &c->d_state->total_updates, &c->d_state->error, (unsigned long long)c->max_updates, kErrUpdatesFull);
   }
   mk.mark(3);
@@ -2141,20 +2190,22 @@ static int front_half(vbx_ctx* c, ScanParams& P, const float* d_xyz, const uint8
 }
 
 // update-record sort + the apply kernels
-static int sort_and_apply(vbx_ctx* c, const ScanParams& P, unsigned long long K, uint32_t n_touched, Marks& mk,
-                          uint64_t* launches) {
+static int sort_and_apply(vbx_ctx* c, Marks& mk, uint64_t* launches) {
   cudaStream_t s = c->stream;
+  const vbx_ctx::Capture* cap = c->cap;
   RecordView rv;
   {
     // K and the number of touched blocks are only known on the device: sort on every bit a
     // record key can have; passes whose digit is uniform are skipped on the device
     const int key_bits = 32;
-    if (c->sort_stream) {
+    if (cap) {
       // pipelined submission: the record sort works on buffers private to this scan, so it leaves
       // the walk stream (which the next scan's ray walk is waiting for)
-      VBX_CUDA(c, cudaEventRecord(c->walked_event, s));
-      VBX_CUDA(c, cudaStreamWaitEvent(c->sort_stream, c->walked_event, 0));
-      s = c->sort_stream;
+      VBX_CUDA(c, cudaEventRecordWithFlags(cap->walked, s, cudaEventRecordExternal));
+      VBX_CUDA(c, cudaEventRecord(cap->edge[0], s));
+      VBX_CUDA(c, cudaStreamWaitEvent(cap->sort, cap->edge[0], 0));
+      VBX_CUDA(c, cudaStreamWaitEvent(cap->sort, cap->prev_sorted, cudaEventWaitExternal));
+      s = cap->sort;
       c->stream = s;
     }
     if (int rc = own_sort<uint32_t>(c, 1, c->ckeys[0], c->cvals[0], c->ckeys[1], c->cvals[1], &c->d_state->total_updates,
@@ -2176,52 +2227,77 @@ static int sort_and_apply(vbx_ctx* c, const ScanParams& P, unsigned long long K,
   lr.keep = c->keep_bits;
   lr.cap = c->max_updates / 32 + 1;
   // everything of the apply that does not depend on the map, on the (pipelined: scan-private) sort stream
-  k_apply_prep<<<c->grid_sms * 8, 256, 0, s>>>(P, c->tab, rv, c->ray_a, c->ray_c, lr, c->d_state);
+  k_apply_prep<<<c->grid_sms * 8, 256, 0, s>>>(c->d_args, c->tab, rv, c->ray_a, c->ray_c, lr, c->d_state);
   mk.mark(6);
-  if (c->apply_stream) {
-    // pipelined submission: the apply kernel runs on its own stream behind the sort, so the
-    // next scan's ray walk can start while this scan's voxels are still being written
-    VBX_CUDA(c, cudaEventRecord(c->sorted_event, s));
-    VBX_CUDA(c, cudaStreamWaitEvent(c->apply_stream, c->sorted_event, 0));
-    s = c->apply_stream;
+  if (cap) {
+    // pipelined submission: the apply kernel runs behind the previous scan's apply, so the next scan's
+    // ray walk can start while this scan's voxels are still being written
+    VBX_CUDA(c, cudaEventRecordWithFlags(cap->sorted, s, cudaEventRecordExternal));
+    VBX_CUDA(c, cudaEventRecord(cap->edge[1], s));
+    VBX_CUDA(c, cudaStreamWaitEvent(cap->apply, cap->edge[1], 0));
+    VBX_CUDA(c, cudaStreamWaitEvent(cap->apply, cap->prev_applied, cudaEventWaitExternal));
+    s = cap->apply;
   }
-  k_apply<<<c->grid_sms * 8, 32 * kApplyWarps, 0, s>>>(P, c->tab, rv, lr, c->d_state);
+  k_apply<<<c->grid_sms * 8, 32 * kApplyWarps, 0, s>>>(c->d_args, c->tab, rv, lr, c->d_state);
+  if (cap) VBX_CUDA(c, cudaEventRecordWithFlags(cap->applied, s, cudaEventRecordExternal));
   mk.mark(7);
   *launches += 2;
   return VBX_OK;
 }
 
 template <typename KeyT>
-static int back_half(vbx_ctx* c, const ScanParams& P, const KeyT* keys, unsigned long long K, uint32_t n_touched,
-                     Marks& mk, uint64_t* launches) {
+static int back_half(vbx_ctx* c, const ScanParams& P, const KeyT* keys, Marks& mk, uint64_t* launches) {
   cudaStream_t s = c->stream;
-  const uint32_t n = P.n;
   if (P.kind == VBX_MERGED && P.single_walk) {
     // a few thousand bundles of 100-300 steps: one warp per ray
-    k_rays_emit_warp<KeyT><<<c->grid_sms * 8, 128, 0, s>>>(P, c->tab, keys, c->ray_list, c->head_list, c->ray_p, c->cnt, c->off,
-                                                   c->ckeys[0], c->cvals[0], c->d_state);
+    k_rays_emit_warp<KeyT><<<c->grid_sms * 8, 128, 0, s>>>(c->d_args, c->tab, keys, c->ray_list, c->head_list, c->ray_p,
+                                                           c->cnt, c->off, c->ckeys[0], c->cvals[0], c->d_state);
   } else {
-    k_rays_emit<KeyT><<<grid_for(n, 128), 128, 0, s>>>(P, c->tab, keys, c->ray_list, c->head_list, c->ray_p, c->cnt, c->off,
-                                                        c->ckeys[0], c->cvals[0], c->d_state);
+    k_rays_emit<KeyT><<<grid_for(c->max_points, 128), 128, 0, s>>>(c->d_args, c->tab, keys, c->ray_list, c->head_list,
+                                                                   c->ray_p, c->cnt, c->off, c->ckeys[0], c->cvals[0],
+                                                                   c->d_state);
   }
   mk.mark(5);
-  k_assign<<<grid_for(std::max<uint32_t>(c->tab.max_blocks, 1024), 256), 256, 0, s>>>(
-      c->tab, c->d_nblocks + c->nb_cur, c->d_nblocks + (c->nb_cur ^ 1), c->sort_plan[1], c->d_state);
+  k_assign<<<grid_for(std::max<uint32_t>(c->tab.max_blocks, 1024), 256), 256, 0, s>>>(c->tab, c->d_args, c->d_nblocks,
+                                                                                      c->sort_plan[1], c->d_state);
   c->nb_cur ^= 1;
   mk.mark(4);
   *launches += 2;
-  return sort_and_apply(c, P, K, n_touched, mk, launches);
+  return sort_and_apply(c, mk, launches);
+}
+
+static void fill_args(const vbx_ctx* c, const ScanParams& P, const float* xyz, const uint8_t* rgba, ScanArgs* a) {
+  a->P = P;
+  a->xyz = xyz;
+  a->rgba = rgba;
+  a->n = P.n;
+  a->n_scan = P.n + 1;
+  a->nb_cur = (uint32_t)c->nb_cur;
+}
+
+// The synchronous calls' argument block goes through hand-off set 0's page-locked copy: the host writes it
+// only when the stream has finished every earlier upload.
+static int upload_args(vbx_ctx* c, const ScanArgs& a) {
+  *c->h_args = a;
+  VBX_CUDA(c, cudaMemcpyAsync(c->d_args, c->h_args, sizeof(ScanArgs), cudaMemcpyHostToDevice, c->stream));
+  return VBX_OK;
+}
+
+int alloc_scan_args(vbx_ctx* c, vbx_ctx::ScratchSet& S) {
+  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&S.d_args), sizeof(ScanArgs)));
+  VBX_CUDA(c, cudaMallocHost(reinterpret_cast<void**>(&S.h_args), sizeof(ScanArgs)));
+  return VBX_OK;
 }
 
 // The back half of a call whose K exceeds max_updates_per_pass, in passes (see integrate_device).
 template <typename KeyT>
-static int apply_in_passes(vbx_ctx* c, ScanParams P, const KeyT* keys, Marks& mk, uint64_t* launches) {
+static int apply_in_passes(vbx_ctx* c, ScanArgs a, const KeyT* keys, Marks& mk, uint64_t* launches) {
   cudaStream_t s = c->stream;
-  const uint32_t n = P.n;
+  const uint32_t n = a.P.n;
   std::vector<uint32_t> off(n + 1);
   VBX_CUDA(c, cudaMemcpyAsync(off.data(), c->off, (size_t)(n + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));
-  if (P.kind == VBX_MERGED) {
+  if (a.P.kind == VBX_MERGED) {
     // the scan wrote the offsets of the bundles and, at [n], the total; ranks past the last bundle hold nothing
     const uint32_t nr = std::min(c->h_state->n_ray_list, n);
     for (uint32_t i = nr + 1; i < n; ++i) off[i] = off[n];
@@ -2237,12 +2313,15 @@ static int apply_in_passes(vbx_ctx* c, ScanParams P, const KeyT* keys, Marks& mk
     if (hi <= lo) return fail(c, VBX_E_CAPACITY, "a single ray has more updates than max_updates_per_pass");
     const unsigned long long kp = (unsigned long long)off[hi] - off[lo];
     if (kp > 0) {
-      P.emit_lo = lo;
-      P.emit_hi = hi;
-      P.emit_base = off[lo];
+      a.P.emit_lo = lo;
+      a.P.emit_hi = hi;
+      a.P.emit_base = off[lo];
+      a.nb_cur = (uint32_t)c->nb_cur;
+      VBX_CUDA(c, cudaStreamSynchronize(s));  // (the previous pass has read its arguments)
+      if (int rc = upload_args(c, a)) return rc;
       k_pass_begin<<<1, 1, 0, s>>>(c->d_state, kp);
       *launches += 1;
-      if (int rc = back_half<KeyT>(c, P, keys, kp, 0, mk, launches)) return rc;
+      if (int rc = back_half<KeyT>(c, a.P, keys, mk, launches)) return rc;
       ++passes;
     }
     lo = hi;
@@ -2324,6 +2403,9 @@ int integrate_device(vbx_ctx* c, int kind, const float q[4], const float t[3], c
     c->last_ms = 0.f;
     return VBX_OK;
   }
+  ScanArgs a;
+  fill_args(c, P, d_xyz, d_rgba, &a);
+  if (int rc = upload_args(c, a)) return rc;
   const int TB = 256;
   Marks mk;
   mk.c = c;
@@ -2348,10 +2430,10 @@ int integrate_device(vbx_ctx* c, int kind, const float q[4], const float t[3], c
   const uint64_t* keys64 = nullptr;
   unsigned long long K = 0;
   uint32_t n_touched = 0;
-  if (int rc = front_half<uint64_t>(c, P, d_xyz, d_rgba, order, mk, &launches, &keys64)) return rc;
+  if (int rc = front_half<uint64_t>(c, P, order, mk, &launches, &keys64)) return rc;
   {
     // own sort: K stays on the device, the whole call is enqueued without a host round trip
-    if (int rc = back_half<uint64_t>(c, P, keys64, 0, 0, mk, &launches)) return rc;
+    if (int rc = back_half<uint64_t>(c, P, keys64, mk, &launches)) return rc;
     VBX_CUDA(c, cudaEventRecord(c->ev1, s));
     VBX_CUDA(c, cudaMemcpyAsync(c->h_state, c->d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
     VBX_CUDA(c, cudaStreamSynchronize(s));
@@ -2361,7 +2443,7 @@ int integrate_device(vbx_ctx* c, int kind, const float q[4], const float t[3], c
       // contiguous ray-slot ranges: every voxel still sees its updates in ray-rank order, so
       // the result is the one-pass result bit for bit.
       chunk_blocks_before = c->n_blocks;
-      if (int rc = apply_in_passes<uint64_t>(c, P, keys64, mk, &launches)) return rc;
+      if (int rc = apply_in_passes<uint64_t>(c, a, keys64, mk, &launches)) return rc;
       chunked = true;
       VBX_CUDA(c, cudaEventRecord(c->ev1, s));
       VBX_CUDA(c, cudaMemcpyAsync(c->h_state, c->d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
@@ -2399,16 +2481,191 @@ int integrate_device(vbx_ctx* c, int kind, const float q[4], const float t[3], c
 
 // ------------------------------------------------------------- asynchronous submission
 // integratePointCloud without the host round trip: the call enqueues the scan and returns.  A scan
-// passes through three stages on separate streams:
-//   front   keys, bundle sort, bundle fold, record offsets -- touches nothing of the map; two front
-//           lanes alternate, so two front halves can run side by side
-//   walk    ray walk with block creation, slot assignment (stream_e)
-//   sort    record sort on scan-private buffers (two sort streams alternate)
-//   apply   the per-voxel updates (main stream)
-// Stages that touch the map run in submission order (one stream each; the walk of scan i+1 only
-// inserts new hash entries and never moves existing ones, so it can overlap the apply of scan i).
-// Up to kSets scans are in flight, each with its own hand-off buffers; results (counters, errors)
-// of a scan are collected when its set is reused or at the next synchronous call / vbx_sync.
+// passes through four stages:
+//   front   keys, bundle sort, bundle fold, record offsets -- touches nothing of the map; the front
+//           lanes alternate, so several front halves can run side by side
+//   walk    ray walk with block creation, slot assignment
+//   sort    record sort and apply preparation on scan-private buffers
+//   apply   the per-voxel updates
+// Stages that touch the map run in submission order (the walk of scan i+1 only inserts new hash
+// entries and never moves existing ones, so it can overlap the apply of scan i).  Up to kSets scans
+// are in flight, each with its own hand-off buffers; results (counters, errors) of a scan are
+// collected when its set is reused or at the next synchronous call / vbx_sync.
+//
+// A scan is one launch of a CUDA graph: the kernels and hand-offs the enqueue code above issues,
+// captured once per (hand-off set, front lane, kind) and kept until vbx_destroy.  What changes from
+// scan to scan is in the set's argument block (uploaded by the graph's first node) or in three kernel
+// nodes updated in place (the two sorts' grids, k_bundle_order's form and shared memory).  The order between
+// scans is carried by events: the front half waits for the lane's previous front half, the walk for
+// the previous scan's walk, the record sort for the one two scans back, the apply for the previous
+// scan's apply.  An event-record node of an earlier launched graph is the event's most recent record
+// for a later one (tests/test_async_graph_gpu.py checks the maps bit for bit against synchronous calls).
+static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& F, const ScanParams& P,
+                        vbx_ctx::ScanGraph& G) {
+  const int k = (int)(&S - c->set), sets = c->sets_in_use;
+  const vbx_ctx::ScratchSet& prev = c->set[(k + sets - 1) % sets];
+  const vbx_ctx::ScratchSet& prev2 = c->set[(k + 2 * sets - 2) % sets];
+  const vbx_ctx::Capture cap{c->stream_s, c->stream_main, S.walked, S.sorted, S.applied, prev2.sorted, prev.applied,
+                             {c->cap_ev[2], c->cap_ev[3]}};
+  cudaStream_t o = S.stream;
+  uint64_t launches = 0;
+  Marks mk;  // (stage profiling is off while a graph is captured)
+  mk.c = c;
+  mk.s = F.stream;
+  auto enqueue = [&]() -> int {
+    VBX_CUDA(c, cudaMemcpyAsync(S.d_args, S.h_args, sizeof(ScanArgs), cudaMemcpyHostToDevice, o));
+    VBX_CUDA(c, cudaStreamWaitEvent(o, S.copy_done, cudaEventWaitExternal));  // a host cloud's copy
+    VBX_CUDA(c, cudaStreamWaitEvent(o, F.done, cudaEventWaitExternal));       // the lane's previous front half
+    // ---- front half on the lane's stream
+    VBX_CUDA(c, cudaEventRecord(c->cap_ev[0], o));
+    VBX_CUDA(c, cudaStreamWaitEvent(F.stream, c->cap_ev[0], 0));
+    c->stream = F.stream;
+    VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), F.stream));
+    if (c->timeline) VBX_CUDA(c, cudaEventRecordWithFlags(S.front_start, F.stream, cudaEventRecordExternal));
+    const uint64_t* keys64 = nullptr;
+    if (int rc = front_half<uint64_t>(c, P, nullptr, mk, &launches, &keys64)) return rc;
+    VBX_CUDA(c, cudaEventRecordWithFlags(F.done, F.stream, cudaEventRecordExternal));
+    if (c->timeline) VBX_CUDA(c, cudaEventRecordWithFlags(S.front_done, F.stream, cudaEventRecordExternal));
+    // ---- walk, record sort and apply (sort_and_apply hands off between their streams)
+    VBX_CUDA(c, cudaEventRecord(c->cap_ev[1], F.stream));
+    VBX_CUDA(c, cudaStreamWaitEvent(c->stream_e, c->cap_ev[1], 0));
+    VBX_CUDA(c, cudaStreamWaitEvent(c->stream_e, prev.walked, cudaEventWaitExternal));
+    c->stream = c->stream_e;
+    c->cap = &cap;
+    // Scans run their map-touching stages in submission order.  A scan that cannot be applied
+    // asynchronously (more update records than one pass holds) raises the context's hold flag here;
+    // every scan queued behind it then skips its back half, and the host redoes all of them
+    // synchronously, in order, from the retained inputs (recover_async, vbx_capi.cu).
+    k_back_begin<<<1, 1, 0, c->stream_e>>>(S.d_state, c->d_hold);
+    launches += 1;
+    if (int rc = back_half<uint64_t>(c, P, keys64, mk, &launches)) return rc;
+    VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, cap.apply));
+    // every stream of the capture joins its origin
+    const cudaStream_t joined[4] = {F.stream, c->stream_e, c->stream_s, c->stream_main};
+    for (int j = 0; j < 4; ++j) {
+      VBX_CUDA(c, cudaEventRecord(c->cap_ev[4 + j], joined[j]));
+      VBX_CUDA(c, cudaStreamWaitEvent(o, c->cap_ev[4 + j], 0));
+    }
+    return VBX_OK;
+  };
+  VBX_CUDA(c, cudaStreamBeginCapture(o, cudaStreamCaptureModeThreadLocal));
+  int rc = enqueue();
+  cudaGraph_t g = nullptr;
+  const cudaError_t e = cudaStreamEndCapture(o, &g);
+  c->cap = nullptr;
+  c->stream = c->stream_main;
+  if (rc == VBX_OK && e != cudaSuccess) rc = cuda_fail(c, e, "cudaStreamEndCapture");
+  // Per-node stage priorities (apply > walk > sort > front, as the streams of the unpipelined stages had)
+  // and the nodes whose launch shape follows the scan or the hints.
+  cudaGraphNode_t point_sort = nullptr, record_sort = nullptr, order = nullptr;
+  cudaKernelNodeParams pp = {}, rp = {}, op = {};
+  if (rc == VBX_OK) {
+    const int walk_prio = std::min(c->prio_lo, c->prio_hi + 1), sort_prio = std::min(c->prio_lo, c->prio_hi + 2);
+    size_t nn = 0;
+    cudaGraphGetNodes(g, nullptr, &nn);
+    std::vector<cudaGraphNode_t> nodes(nn);
+    cudaGraphGetNodes(g, nodes.data(), &nn);
+    for (cudaGraphNode_t nd : nodes) {
+      cudaGraphNodeType ty;
+      cudaKernelNodeParams kp;
+      if (cudaGraphNodeGetType(nd, &ty) != cudaSuccess || ty != cudaGraphNodeTypeKernel ||
+          cudaGraphKernelNodeGetParams(nd, &kp) != cudaSuccess) {
+        continue;
+      }
+      cudaLaunchAttributeValue prio = {};
+      prio.priority = c->prio_lo;
+      if (kp.func == (void*)k_back_begin || kp.func == (void*)k_rays_emit_warp<uint64_t> ||
+          kp.func == (void*)k_rays_emit<uint64_t> || kp.func == (void*)k_assign) {
+        prio.priority = walk_prio;
+      } else if (kp.func == (void*)k_sort<uint32_t> || kp.func == (void*)k_apply_prep) {
+        prio.priority = sort_prio;
+      } else if (kp.func == (void*)k_apply) {
+        prio.priority = c->prio_hi;
+      }
+      if (cudaGraphKernelNodeSetAttribute(nd, cudaLaunchAttributePriority, &prio) != cudaSuccess) {
+        rc = fail(c, VBX_E_CUDA, "cudaGraphKernelNodeSetAttribute(priority)");
+      }
+      if (kp.func == (void*)k_sort<uint64_t>) {
+        point_sort = nd;
+        pp = kp;
+      } else if (kp.func == (void*)k_sort<uint32_t>) {
+        record_sort = nd;
+        rp = kp;
+      } else if (kp.func == (void*)k_bundle_order) {
+        order = nd;
+        op = kp;
+      }
+    }
+    if (rc == VBX_OK && (!record_sort || (P.kind == VBX_MERGED) != (order != nullptr && point_sort != nullptr))) {
+      rc = fail(c, VBX_E_CUDA, "captured scan graph: sort / bundle order node not found");
+    }
+  }
+  cudaGraphExec_t x = nullptr;
+  if (rc == VBX_OK) {
+    const cudaError_t ei = cudaGraphInstantiateWithFlags(&x, g, cudaGraphInstantiateFlagUseNodePriority);
+    if (ei != cudaSuccess) rc = cuda_fail(c, ei, "cudaGraphInstantiateWithFlags");
+  }
+  if (rc == VBX_OK) {
+    // (otherwise the graph's first launch uploads it, in the middle of a stream of scans)
+    const cudaError_t eu = cudaGraphUpload(x, o);
+    if (eu != cudaSuccess) rc = cuda_fail(c, eu, "cudaGraphUpload");
+  }
+  if (rc != VBX_OK) {
+    if (x) cudaGraphExecDestroy(x);
+    if (g) cudaGraphDestroy(g);
+    return rc;
+  }
+  G.graph = g;
+  G.exec = x;
+  G.launches = launches;
+  G.point_sort = point_sort;
+  G.point_grid = pp.gridDim.x;
+  G.record_sort = record_sort;
+  G.record_grid = rp.gridDim.x;
+  G.order = order;
+  G.order_grid = op.gridDim.x;
+  G.order_smem = op.sharedMemBytes;
+  return VBX_OK;
+}
+
+static int set_grid(vbx_ctx* c, vbx_ctx::ScanGraph& G, cudaGraphNode_t node, unsigned int grid, unsigned int* now) {
+  if (grid == *now) return VBX_OK;
+  cudaKernelNodeParams p;
+  VBX_CUDA(c, cudaGraphKernelNodeGetParams(node, &p));
+  p.gridDim.x = grid;
+  VBX_CUDA(c, cudaGraphExecKernelNodeSetParams(G.exec, node, &p));
+  *now = grid;
+  return VBX_OK;
+}
+
+// Brings the kernel nodes of a scan graph whose launch shape varies up to date (a no-op unless it moved):
+// the point sort's grid (a grid larger than the scan's tiles keeps blocks waiting between passes), the
+// record sort's grid, k_bundle_order's form (grid) and shared memory.
+static int update_scan_graph(vbx_ctx* c, vbx_ctx::ScanGraph& G, uint32_t n) {
+  if (G.point_sort) {
+    if (int rc = set_grid(c, G, G.point_sort, sort_grid(c, 0, n), &G.point_grid)) return rc;
+  }
+  if (int rc = set_grid(c, G, G.record_sort, sort_grid(c, 1, c->record_hint), &G.record_grid)) return rc;
+  if (G.order) {
+    const OrderLaunch o = order_launch(c, n);
+    if (o.grid != G.order_grid || o.smem_bytes != G.order_smem) {
+      cudaKernelNodeParams p;
+      VBX_CUDA(c, cudaGraphKernelNodeGetParams(G.order, &p));
+      uint32_t smem_words = (uint32_t)(o.smem_bytes / 4);
+      void* args[6];
+      std::copy(p.kernelParams, p.kernelParams + 6, args);
+      args[2] = &smem_words;
+      p.kernelParams = args;
+      p.gridDim.x = o.grid;
+      p.sharedMemBytes = (unsigned int)o.smem_bytes;
+      VBX_CUDA(c, cudaGraphExecKernelNodeSetParams(G.exec, G.order, &p));
+      G.order_grid = o.grid;
+      G.order_smem = o.smem_bytes;
+    }
+  }
+  return VBX_OK;
+}
+
 int integrate_async(vbx_ctx* c, int kind, const float q[4], const float t[3], const float* xyz, const uint8_t* rgba,
                     uint64_t n64, int freespace, int on_device) {
   if (kind < VBX_SIMPLE || kind > VBX_FAST) return fail(c, VBX_E_INVALID, "Unknown TSDF integrator type");
@@ -2432,8 +2689,8 @@ int integrate_async(vbx_ctx* c, int kind, const float q[4], const float t[3], co
   if (int rc = ensure_async(c)) return rc;
   const uint32_t n = (uint32_t)n64;
   const int k = (int)(c->async_seq % c->sets_in_use);
+  const int l = (int)(c->async_seq % c->lanes_in_use);
   vbx_ctx::ScratchSet& S = c->set[k];
-  vbx_ctx::FrontLane& F = c->lane[c->async_seq % c->lanes_in_use];
   const auto t_enter = std::chrono::steady_clock::now();
   if (S.in_flight) {  // bounded run-ahead: wait for the scan that used this hand-off set
     VBX_CUDA(c, cudaEventSynchronize(S.back_done));
@@ -2445,20 +2702,9 @@ int integrate_async(vbx_ctx* c, int kind, const float q[4], const float t[3], co
     }
   }
   select_set(c, k);
-  select_lane(c, (int)(c->async_seq % c->lanes_in_use));
+  select_lane(c, l);
   ScanParams P;
   fill_params(c, kind, q, t, n, freespace, P);
-  uint64_t launches = 0;
-  Marks mk;
-  mk.c = c;
-  mk.s = F.stream;
-  const bool profiling = c->profiling;
-  c->profiling = false;  // stage events would serialise the streams
-  int rc = VBX_OK;
-  // ---- front half on this scan's front lane
-  c->stream = F.stream;
-  c->apply_stream = nullptr;
-  c->sort_stream = nullptr;
   const float* dx = xyz;
   const uint8_t* dr = rgba;
   if (!on_device) {
@@ -2467,59 +2713,49 @@ int integrate_async(vbx_ctx* c, int kind, const float q[4], const float t[3], co
     cudaStream_t sc = (c->async_seq & 1u) ? c->stream_c2 : c->stream_c;
     if (cudaMemcpyAsync(S.d_xyz, xyz, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, sc) != cudaSuccess ||
         cudaMemcpyAsync(S.d_rgba, rgba, (size_t)n * 4, cudaMemcpyHostToDevice, sc) != cudaSuccess ||
-        cudaEventRecord(S.copy_done, sc) != cudaSuccess ||
-        cudaStreamWaitEvent(F.stream, S.copy_done, 0) != cudaSuccess) {
-      rc = fail(c, VBX_E_CUDA, "asynchronous host-to-device copy failed");
+        cudaEventRecord(S.copy_done, sc) != cudaSuccess) {
+      return fail(c, VBX_E_CUDA, "asynchronous host-to-device copy failed");
     }
     dx = S.d_xyz;
     dr = S.d_rgba;
   }
-  const uint64_t* keys64 = nullptr;
-  if (rc == VBX_OK && cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), F.stream) != cudaSuccess) {
-    rc = fail(c, VBX_E_CUDA, "cudaMemsetAsync");
-  }
-  if (rc == VBX_OK && c->timeline) cudaEventRecord(S.front_start, F.stream);
-  if (rc == VBX_OK) {
-    rc = front_half<uint64_t>(c, P, dx, dr, nullptr, mk, &launches, &keys64);
-  }
-  if (rc == VBX_OK && cudaEventRecord(S.front_done, F.stream) != cudaSuccess) rc = fail(c, VBX_E_CUDA, "cudaEventRecord");
-  // ---- walk + record sort on stream_e, apply on the main stream
-  c->stream = c->stream_e;
-  c->sort_stream = c->stream_s[c->async_seq % vbx_ctx::kSortStreams];
-  c->walked_event = S.walked;
-  c->apply_stream = c->stream_main;
-  c->sorted_event = S.sorted;
-  mk.s = c->stream_e;
-  if (rc == VBX_OK && cudaStreamWaitEvent(c->stream_e, S.front_done, 0) != cudaSuccess) {
-    rc = fail(c, VBX_E_CUDA, "cudaStreamWaitEvent");
-  }
-  if (rc == VBX_OK) {
-    // Scans run their map-touching stages in submission order on this stream.  A scan that cannot be
-    // applied asynchronously (more update records than one pass holds) raises the context's hold
-    // flag here; every scan queued behind it then skips its back half, and the host redoes all of
-    // them synchronously, in order, from the retained inputs (recover_async, vbx_capi.cu).
-    if (rc == VBX_OK) {
-      k_back_begin<<<1, 1, 0, c->stream_e>>>(S.d_state, c->d_hold);
-      launches += 1;
-      rc = back_half<uint64_t>(c, P, keys64, 0, 0, mk, &launches);
+  // the set's previous scan has finished (back_done), so its page-locked argument block is free
+  fill_args(c, P, dx, dr, S.h_args);
+  const int nb = c->nb_cur;
+  const int variant = kind == VBX_MERGED ? vbx_ctx::kGraphMerged : vbx_ctx::kGraphSimple;
+  vbx_ctx::ScanGraph& G = S.graph[l][variant];
+  int rc = VBX_OK;
+  // The pipeline runs the kernels of several scans at once (front halves, a walk, a record sort, an apply):
+  // a persistent grid sized for the whole GPU only holds SM slots that the other scans' kernels need.  The
+  // graphs' grids are sized for a quarter of the SMs (DESIGN.md §5b: the pace against the grid scale).
+  const unsigned int full_sms = c->grid_sms;
+  c->grid_sms = std::max(1u, full_sms / 4);
+  if (!G.exec) {
+    // the first scan of its kind captures the graphs of every (set, lane) pair the submission order
+    // reaches (set = seq % sets, lane = seq % lanes), so that no later scan waits for a capture
+    const bool profiling = c->profiling;
+    c->profiling = false;  // stage events would serialise the streams
+    const int pairs = std::lcm(c->sets_in_use, c->lanes_in_use);
+    for (int j = 0; j < pairs && rc == VBX_OK; ++j) {
+      const int kj = j % c->sets_in_use, lj = j % c->lanes_in_use;
+      select_set(c, kj);
+      select_lane(c, lj);
+      rc = capture_scan(c, c->set[kj], c->lane[lj], P, c->set[kj].graph[lj][variant]);
     }
+    select_set(c, k);
+    select_lane(c, l);
+    c->profiling = profiling;
   }
-  // the status block travels on a stream of its own: a copy between two scans' apply kernels would make the
-  // apply stream (the pace setter of the pipeline) hop between the compute and the copy engine for every scan
-  if (rc == VBX_OK && (cudaEventRecord(S.applied, c->stream_main) != cudaSuccess ||
-                       cudaStreamWaitEvent(c->stream_h, S.applied, 0) != cudaSuccess ||
-                       cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, c->stream_h) != cudaSuccess ||
-                       cudaEventRecord(S.back_done, c->stream_h) != cudaSuccess)) {
-    rc = fail(c, VBX_E_CUDA, "enqueueing the result read-back failed");
+  if (rc == VBX_OK) rc = update_scan_graph(c, G, n);
+  c->grid_sms = full_sms;
+  if (rc == VBX_OK && (cudaGraphLaunch(G.exec, S.stream) != cudaSuccess || cudaEventRecord(S.back_done, S.stream) != cudaSuccess)) {
+    rc = fail(c, VBX_E_CUDA, "launching the scan's graph failed");
   }
-  c->profiling = profiling;
-  c->stream = c->stream_main;
-  c->apply_stream = nullptr;
-  c->sort_stream = nullptr;
+  c->nb_cur = rc == VBX_OK ? nb ^ 1 : nb;  // k_assign of the scan moves the block count to the other word
   if (rc != VBX_OK) return rc;
   S.in_flight = true;
   S.kind = kind;
-  S.launches = launches;
+  S.launches = G.launches;
   S.seq = c->async_seq;
   S.redo = false;
   std::memcpy(S.q, q, sizeof(S.q));
@@ -2529,7 +2765,7 @@ int integrate_async(vbx_ctx* c, int kind, const float q[4], const float t[3], co
   S.in_xyz = dx;   // (the set's private copy of a host cloud, or the caller's device buffers)
   S.in_rgba = dr;
   c->async_submit_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t_enter).count();
-  c->launches += launches;
+  c->launches += G.launches;
   c->async_seq += 1;
   if (c->deferred_rc) {
     rc = c->deferred_rc;
@@ -2627,7 +2863,7 @@ int debug_scan(vbx_ctx* c, const uint32_t* in, uint32_t n, uint32_t* out) {
   const uint32_t tiles = (n + kScanTile - 1) / kScanTile;
   VBX_CUDA(c, cudaMemsetAsync(c->scan_status, 0, (size_t)(tiles + 1) * sizeof(uint32_t), s));
   if (n) {
-    k_exclusive_scan<<<std::min<uint32_t>(tiles, c->grid_sms * 4), kSortThreads, 0, s>>>(c->cnt, nullptr, nullptr, c->off, n,
+    k_exclusive_scan<<<std::min<uint32_t>(tiles, c->grid_sms * 4), kSortThreads, 0, s>>>(c->cnt, nullptr, nullptr, c->off, nullptr, n,
                                                                                c->scan_status + 1, c->scan_status, nullptr,
                                                                                nullptr, nullptr, 0ull, 0u);
   }
