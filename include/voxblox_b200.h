@@ -356,6 +356,26 @@ VBX_API int vbx_debug_async_timeline(vbx_ctx* ctx, uint64_t* seq, float* ms, int
  * with LongIndexHash hashes[e]; out[p] = the element at iteration position p.  force_global != 0 uses
  * the global-memory tables even when the shared-memory ones would fit. */
 VBX_API int vbx_debug_bundle_order(vbx_ctx* ctx, const uint32_t* hashes, uint32_t n, int force_global, uint32_t* out);
+/* Test hook for the TSDF apply (the record sort, k_apply_prep and k_apply of every integrate call):
+ * applies n caller-given updates to blocks already in the TSDF layer.  Update r goes to voxel
+ * rec_voxel[r] (< voxels_per_side^3) of block idx3[3 * rec_block[r] ..] (rec_block[r] < n_blocks) with
+ * the final sdf and weight updateTsdfVoxel uses (tsdf_integrator.cc:186-208) and colour rgba[4r ..];
+ * a voxel's updates are applied in the order given, with the config's truncation and max_weight.
+ * Block updated() bits are not touched.  VBX_E_INVALID: n > max_updates_per_pass, a block that is
+ * not in the TSDF layer or is listed twice, an index out of range.  paths (may be NULL) = the apply-path counts below. */
+VBX_API int vbx_debug_apply(vbx_ctx* ctx, const int32_t* idx3, uint32_t n_blocks, uint64_t n, const uint32_t* rec_block,
+                            const uint32_t* rec_voxel, const float* sdf, const float* weight, const uint8_t* rgba,
+                            uint64_t paths[16]);
+/* Counting the apply's paths costs a little on every call, so integrate calls count them only after
+ * vbx_debug_count_apply_paths(ctx, 1) (off by default); vbx_debug_apply always counts. */
+VBX_API int vbx_debug_count_apply_paths(vbx_ctx* ctx, int enabled);
+/* How often each path of the apply ran in the last synchronous integrate call (summed over its passes),
+ * the last collected asynchronous scan, or vbx_debug_apply (zero for calls made with counting off): [0] voxel runs longer than 32 updates (one
+ * warp each) [1] ... cut short at rest (+T, max_weight) [2..4] 128-record steps decided in one go:
+ * weight saturated / integer warp scan / prefix sum [5..8] 32-record chunks decided fast: saturated /
+ * unit weights / prefix sum / clamped sequential chain [9] chunks applied update by update [10] runs of
+ * at most 32 updates [11] ... that continue past their 256-record tile [12..15] zero. */
+VBX_API int vbx_debug_apply_paths(const vbx_ctx* ctx, uint64_t out[16]);
 VBX_API int vbx_timer_start(vbx_ctx* ctx);
 VBX_API int vbx_timer_stop_ms(vbx_ctx* ctx, float* ms);
 VBX_API int vbx_set_stage_profiling(vbx_ctx* ctx, int enabled);

@@ -21,6 +21,7 @@ from tests import test_icp_gpu as ti  # noqa: E402
 from tests import test_merged_reference_gpu as tm  # noqa: E402
 from tests import test_mesh_cpu as tmc  # noqa: E402
 from tests import test_oracle_pin as to  # noqa: E402
+from tests import test_tsdf_edges_gpu as tte  # noqa: E402
 from tests import test_tsdf_ground_truth_gpu as tg  # noqa: E402
 from tests.golden import reference_pins as pins  # noqa: E402
 
@@ -38,6 +39,8 @@ def cases():
         out[f"esdf/{key}"] = lambda lib, k=key: te.reference_side(k, lib)[2]
     for key in teo.PIN_KEYS:
         out[f"esdf_options/{key}"] = lambda lib, k=key: teo.reference_side(k, lib)[2]
+    for key in tte.PIN_KEYS:
+        out[f"tsdf_edges/{key}"] = lambda lib, k=key: tte.reference_side(k, lib)[3]
     for key in tg.PIN_KEYS:
         out[f"tsdf_ground_truth/{key}"] = lambda lib, k=key: tg.reference_side(k, lib)[1]
     for key in ti.PIN_KEYS:

@@ -28,11 +28,14 @@ def _run(kind, scans, voxel_size, trunc, order, **cfg_kw):
 
 
 def _assert_parity(rep):
+    """Simple and Merged reproduce the reference bit for bit (DESIGN.md section 0)."""
     assert rep["blocks_equal"], rep
     assert rep["observed_equal"], rep
     assert rep["max_rel_err"] <= REL_TOL, rep
     assert rep["color_mismatch"] == 0, rep
     assert rep["updated_equal"], rep
+    assert rep["max_rel_err"] == 0.0, rep
+    assert rep["n_bit_exact"] == rep["n_voxels"], rep
 
 
 def test_c1_simple_planar_wall():

@@ -135,7 +135,7 @@ EXPORTS = ["vbx_create", "vbx_destroy", "vbx_last_error", "vbx_version", "vbx_ge
            "vbx_esdf_create", "vbx_esdf_update", "vbx_esdf_get_counters", "vbx_sync",
            "vbx_timer_start", "vbx_timer_stop_ms", "vbx_set_stage_profiling", "vbx_get_stage_ms",
            "vbx_host_alloc", "vbx_host_free", "vbx_host_copy_ms", "vbx_block_owner",
-           "vbx_debug_sort", "vbx_debug_scan", "vbx_debug_bundle_order", "vbx_debug_async_timeline", "vbx_tsdf_integrate_async", "vbx_esdf_update_blocks", "vbx_esdf_set_max_distance",
+           "vbx_debug_sort", "vbx_debug_scan", "vbx_debug_bundle_order", "vbx_debug_apply", "vbx_debug_apply_paths", "vbx_debug_count_apply_paths", "vbx_debug_async_timeline", "vbx_tsdf_integrate_async", "vbx_esdf_update_blocks", "vbx_esdf_set_max_distance",
            "vbx_esdf_set_full_euclidean", "vbx_esdf_get_config", "vbx_esdf_add_robot_position", "vbx_esdf_clear", "vbx_mesh_generate", "vbx_mesh_download", "vbx_icp_run", "vbx_icp_run_device", "vbx_mirror_updated", "vbx_serialize_updated", "vbx_deserialize_blocks", "vbx_save_layer", "vbx_load_layer",
            "vbx_proto_encode_layer", "vbx_proto_encode_block", "vbx_proto_decode_block"]
 
@@ -173,6 +173,12 @@ def load_library():
     lib.vbx_tsdf_integrate_async.argtypes = [vp, i32, vp, vp, vp, vp, u64, i32, i32]
     lib.vbx_get_counters.restype = i32
     lib.vbx_get_counters.argtypes = [vp, vp]
+    lib.vbx_debug_apply.restype = i32
+    lib.vbx_debug_apply.argtypes = [vp, vp, C.c_uint32, u64, vp, vp, vp, vp, vp, vp]
+    lib.vbx_debug_apply_paths.restype = i32
+    lib.vbx_debug_apply_paths.argtypes = [vp, vp]
+    lib.vbx_debug_count_apply_paths.restype = i32
+    lib.vbx_debug_count_apply_paths.argtypes = [vp, i32]
     lib.vbx_esdf_get_counters.restype = i32
     lib.vbx_esdf_get_counters.argtypes = [vp, vp]
     lib.vbx_last_device_ms.restype = i32
@@ -604,6 +610,20 @@ class TsdfIntegratorBase:
                  "blocks_allocated", "valid_points", "kernel_launches", "kernel_launches_total", "refolded_bundles",
                  "refolded_points", "passes", "bundle_key_bits", "async_redone_total", "async_wait_ns_total", "async_submit_ns_total"]
         return {k: int(v) for k, v in zip(names, out)}
+
+    APPLY_PATHS = ["long_runs", "long_rested", "step_saturated", "step_int_scan", "step_prefix", "chunk_saturated",
+                   "chunk_const", "chunk_prefix", "chunk_sequential", "chunk_exact", "short_runs", "short_crossed"]
+
+    def countApplyPaths(self, enabled: bool = True) -> None:
+        """Make later integrate calls count the apply's paths (vbx_debug_count_apply_paths; off by default)."""
+        self._ctx.check(self._ctx.lib.vbx_debug_count_apply_paths(self._ctx.handle, int(bool(enabled))),
+                        "vbx_debug_count_apply_paths")
+
+    def applyPaths(self) -> Dict[str, int]:
+        """How often each arithmetic path of the apply ran in the last call (vbx_debug_apply_paths)."""
+        out = np.zeros(16, dtype=np.uint64)
+        self._ctx.check(self._ctx.lib.vbx_debug_apply_paths(self._ctx.handle, out.ctypes.data), "vbx_debug_apply_paths")
+        return {k: int(v) for k, v in zip(self.APPLY_PATHS, out)}
 
     def lastDeviceMs(self) -> float:
         ms = C.c_float(0)

@@ -17,6 +17,8 @@ int debug_sort(vbx_ctx* c, const void* keys, int key_bytes, uint32_t n, int key_
                uint32_t* vals_out);
 int debug_scan(vbx_ctx* c, const uint32_t* in, uint32_t n, uint32_t* out);
 int debug_bundle_order(vbx_ctx* c, const uint32_t* hashes, uint32_t n, int force_global, uint32_t* out);
+int debug_apply(vbx_ctx* c, const int32_t* idx3, uint32_t nb, uint64_t n, const uint32_t* rec_block,
+                const uint32_t* rec_voxel, const float* sdf, const float* w, const uint8_t* rgba, uint64_t paths[16]);
 int upload_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, const void* voxels,
                   const uint8_t* updated_bits, int serialized);
 int remove_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m);
@@ -78,6 +80,7 @@ void harvest_async(vbx_ctx* c, vbx_ctx::ScratchSet& S) {
   c->counters[6] = S.kind == VBX_MERGED ? h.n_valid_points : (uint64_t)h.n_rays + h.n_clear_rays;
   c->counters[7] = S.launches;
   c->counters[11] = 1;
+  for (int i = 0; i < kApplyPaths; ++i) c->apply_paths[i] = h.apply_paths[i];
   const uint32_t fatal = h.error & kFatalErrors & ~kErrUpdatesFull;
   if (!fatal && (h.error & (kErrUpdatesFull | kSkipped))) {
     // more update records than one pass holds (or queued behind such a scan): nothing was applied;
@@ -708,6 +711,31 @@ int vbx_debug_bundle_order(vbx_ctx* c, const uint32_t* hashes, uint32_t n, int f
   VBX_CUDA(c, cudaSetDevice(c->device));
   VBX_DRAIN(c);
   return debug_bundle_order(c, hashes, n, force_global, out);
+}
+
+int vbx_debug_apply(vbx_ctx* c, const int32_t* idx3, uint32_t n_blocks, uint64_t n, const uint32_t* rec_block,
+                    const uint32_t* rec_voxel, const float* sdf, const float* weight, const uint8_t* rgba,
+                    uint64_t paths[16]) {
+  if (!c || (n_blocks && !idx3) || (n && (!rec_block || !rec_voxel || !sdf || !weight || !rgba))) {
+    return fail(c, VBX_E_INVALID, "null argument");
+  }
+  VBX_CUDA(c, cudaSetDevice(c->device));
+  VBX_DRAIN(c);
+  return debug_apply(c, idx3, n_blocks, n, rec_block, rec_voxel, sdf, weight, rgba, paths);
+}
+
+int vbx_debug_count_apply_paths(vbx_ctx* c, int enabled) {
+  if (!c) return VBX_E_INVALID;
+  VBX_CUDA(c, cudaSetDevice(c->device));
+  VBX_DRAIN(c);  // (scans already queued keep the setting they were submitted with)
+  c->count_apply_paths = enabled != 0;
+  return VBX_OK;
+}
+
+int vbx_debug_apply_paths(const vbx_ctx* c, uint64_t out[16]) {
+  if (!c || !out) return VBX_E_INVALID;
+  std::memcpy(out, c->apply_paths, sizeof(c->apply_paths));
+  return VBX_OK;
 }
 
 int vbx_get_counters(const vbx_ctx* c, uint64_t out[16]) {

@@ -54,6 +54,25 @@ enum : uint32_t {
   kSkipped = 32u,           // not an error: the scan was queued behind a scan that must be redone (vbx_capi.cu)
 };
 
+// The paths of k_apply, counted per call in ScanState::apply_paths (vbx_debug_apply_paths reports them).
+// Each path claims the sequential updateTsdfVoxel result bit for bit; the counts show which of them a
+// call exercised.
+enum ApplyPath : int {
+  kPathLongRun = 0,        // runs longer than kShortRun updates, one warp each
+  kPathLongRested,         // ... of which the rest was skipped: the voxel rests at (+T, max_weight), every later record keeps
+  kPathStepSaturated,      // 4 x 32-record steps decided in one go: weight already at max_weight
+  kPathStepIntScan,        // ... integer weights below 2^24: a warp scan forms the weight chain
+  kPathStepPrefix,         // ... an in-order prefix sum forms it
+  kPathChunkSaturated,     // 32-record chunks decided fast: weight already at max_weight
+  kPathChunkConst,         // ... unit weights on an integer weight below 2^22
+  kPathChunkPrefix,        // ... an in-order prefix sum
+  kPathChunkSequential,    // ... the clamped weight chain, one record after the other
+  kPathChunkExact,         // 32-record chunks applied with the exact per-record update
+  kPathShortRun,           // runs of at most kShortRun updates, one thread each
+  kPathShortCrossed,       // ... that continue past the end of their shared-memory tile
+  kApplyPaths
+};
+
 // Device-resident per-call state; the host reads it back through pinned memory.
 struct ScanState {
   uint32_t n_new;            // hash entries created by this call
@@ -91,9 +110,11 @@ struct ScanState {
   uint32_t rec_key_bits;     // bits an update-record key uses: voxel-in-block bits + bits of the touched ids
   uint32_t esdf_ticket[6];   // ESDF queue kernels: work hand-out counters, rotating like the queue counters ([0..2] raise, [3..5] lower)
   uint32_t tile_ticket;      // k_apply: record tiles of the short runs handed out
-  uint32_t reserved[14];
+  uint32_t apply_paths[12];  // k_apply: how often each arithmetic path ran, summed over the call (ApplyPath)
+  uint32_t reserved[2];
 };
 static_assert(sizeof(ScanState) == 256, "the status block the host reads back is 256 bytes");
+static_assert(sizeof(ScanState::apply_paths) / 4 == kApplyPaths, "one word per apply path");
 
 // The GPU-resident block hash + voxel pools (the device mirror of Layer<T>::block_map_,
 // core/layer.h:30-32,292).
@@ -348,6 +369,8 @@ struct vbx_ctx {
   // reporting
   uint32_t last_passes = 1;  // passes the last synchronous integrate call needed (K > max_updates_per_pass)
   uint64_t counters[16] = {0};
+  uint64_t apply_paths[16] = {0};  // ScanState::apply_paths of the last call whose status reached the host
+  bool count_apply_paths = false;  // k_apply counts its paths (vbx_debug_count_apply_paths; vbx_debug_apply always does)
   uint64_t async_wait_ns = 0, async_submit_ns = 0;  // host time of vbx_tsdf_integrate_async: waiting for a hand-off set / enqueueing
   uint64_t esdf_counters[16] = {0};
   uint64_t shard_front_counters[4] = {0};

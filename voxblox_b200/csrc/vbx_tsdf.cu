@@ -90,6 +90,7 @@ struct ScanArgs {
   unsigned long long n;  // P.n: the point sort's element count
   uint32_t n_scan;       // P.n + 1: positions of the record-offset scan
   uint32_t nb_cur;       // k_assign reads d_nblocks[nb_cur], writes d_nblocks[nb_cur ^ 1]
+  uint32_t count_paths;  // k_apply counts its paths into ScanState::apply_paths (vbx_debug_count_apply_paths)
 };
 
 // MixedThreadSafeIndex::getNextIndexImpl, integrator_utils.cc:54-63
@@ -1572,9 +1573,18 @@ __device__ __forceinline__ Prepared open_prepared(const RecordView& rv) {
 // so "unchanged" is exact, not approximate.  Run heads count the distinct voxels (U) and list the
 // runs longer than kShortRun updates with their [start, end).  Records of blocks this rank does not
 // own (kSkipRecord) sort to the end and are skipped.
+//
+// kGiven (vbx_debug_apply only): a record's value is its ordinal into caller-given sdf / weight / colour
+// arrays instead of a ray id, so that a test can drive the production apply with any update sequence.
+struct GivenRecords {
+  const float* sdf;
+  const float* w;
+  const uint32_t* col;
+};
+template <bool kGiven>
 __global__ void __launch_bounds__(256, 6)
 k_apply_prep(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, const float4* __restrict__ ray_a,
-             const uint2* __restrict__ ray_c, LongRuns lr, ScanState* st) {
+             const uint2* __restrict__ ray_c, LongRuns lr, ScanState* st, GivenRecords given) {
   const ScanParams P = A->P;
   const uint32_t sel = rv.plan ? rv.plan->final_buf : 0u;
   const uint32_t* __restrict__ keys = rv.keys[sel];
@@ -1591,14 +1601,21 @@ k_apply_prep(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, const fl
     bool keep = false, head = false;
     if (key != kSkipRecord) {
       const uint32_t r = vals[e];
-      const float4 ra = ray_a[r];
-      const uint2 rc = ray_c[r];
       const VoxelRef vr = locate_voxel(P, tab, key);
-      const float sdf = sdf_from(vr.vo, ra);
-      const float w = update_weight(sdf, __uint_as_float(rc.y), P.up);
+      float sdf, w;
+      if (kGiven) {
+        sdf = given.sdf[r];
+        w = given.w[r];
+        vals[e] = given.col[r];
+      } else {
+        const float4 ra = ray_a[r];
+        const uint2 rc = ray_c[r];
+        sdf = sdf_from(vr.vo, ra);
+        w = update_weight(sdf, __uint_as_float(rc.y), P.up);
+        vals[e] = rc.x;
+      }
       rec_sdf[e] = sdf;
       rec_w[e] = w;
-      vals[e] = rc.x;
       const float nw = fadd(W, w);
       keep = sdf >= T && !(nw < VBX_EPS) && !(nw < W);
       if (keep) {
@@ -1692,12 +1709,26 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
   const uint32_t n_long = st->n_long;
   const float T = P.up.trunc;
   const bool can_rest = P.up.max_weight >= VBX_EPS;
+  const int wb = threadIdx.x >> 5;
+  // How often each path ran (ApplyPath), only when asked for (ScanArgs::count_paths: tests and diagnostics),
+  // added to the status block once per warp when it leaves.  The long-run paths are decided per warp: lane 0
+  // counts them in the warp's row of s_paths (in shared memory, so that they take no registers from the
+  // chains).  Short runs are counted per lane in two registers.
+  const bool counting = A->count_paths != 0u;
+  __shared__ uint32_t s_paths[kApplyWarps][kApplyPaths];
+  if (counting && lane < kApplyPaths) s_paths[wb][lane] = 0u;
+  __syncwarp();
+  auto count = [&](int path) {
+    if (counting && lane == 0) ++s_paths[wb][path];
+  };
+  uint32_t n_short = 0, n_crossed = 0;
   for (;;) {
     uint32_t q = 0;
     if (lane == 0) q = atomicAdd(&st->long_ticket, 1u);
     q = __shfl_sync(0xffffffffu, q, 0);
     if (q >= n_long) break;
     const unsigned long long start = lr.start[q], end = lr.end[q];
+    count(kPathLongRun);
     const VoxelRef vr = locate_voxel(P, tab, keys[start]);
     TsdfVoxel v = *vr.ptr;
     unsigned long long keep_from = ~0ull;  // found on first need
@@ -1715,7 +1746,10 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
     for (;;) {
       if (can_rest && v.distance == T && v.weight == P.up.max_weight) {
         if (keep_from == ~0ull) keep_from = keep_suffix(lr.keep, start, end, lane);
-        if (j0 >= keep_from) break;
+        if (j0 >= keep_from) {
+          count(kPathLongRested);
+          break;
+        }
       }
       bool in_c[kG];
       float sdf_c[kG], w_c[kG];
@@ -1758,6 +1792,7 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
           float mb[kG];
           float w_end = v.weight;
           bool have = true;
+          int path = kPathStepSaturated;
           if (saturated) {
             // W + w >= max_weight for every w >= 0: the clamp returns max_weight at every step
 #pragma unroll
@@ -1768,6 +1803,7 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
 #pragma unroll
             for (int g = 0; g < kG; ++g) ints = ints && wl[g] == truncf(wl[g]);
             if (__all_sync(0xffffffffu, ints)) {
+              path = kPathStepIntScan;
               // integer-valued weights (use_const_weight: a bundle's weight is its point count) on an
               // integer-valued W, everything below 2^24: every partial sum is exact, so any order gives
               // the in-order chain -- a warp scan per chunk
@@ -1785,6 +1821,7 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
               }
               w_end = base;
             } else {
+              path = kPathStepPrefix;
               float base = v.weight;
 #pragma unroll
               for (int g = 0; g < kG; ++g) {
@@ -1818,6 +1855,7 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
             if (__all_sync(0xffffffffu, keeps_T)) {
               v.weight = w_end;
               step_done = true;
+              count(path);
             }
           }
         }
@@ -1832,6 +1870,7 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
         const bool far_free = !in || sdf >= T;
         bool fast = __all_sync(0xffffffffu, far_free) && v.distance == T;
         float w_end = v.weight;
+        int path = kPathChunkSaturated;
         if (fast) {
           // exact sequential weight chain: W <- min(W + w, max_weight) unless W + w < 1e-6
           float my_before = 0.f;
@@ -1847,11 +1886,13 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
                      __all_sync(0xffffffffu, !in || w == 1.0f)) {
             // constant weights (use_const_weight) on an integer-valued W below 2^22: every partial
             // sum is an integer that float represents exactly, so the in-order chain is W + k
+            path = kPathChunkConst;
             my_before = v.weight + (float)lane;
             w_end = v.weight + (float)cnt;
           } else if (no_clamp) {
             // neither the 1e-6 guard nor the max_weight clamp can fire in this chunk: the
             // chain is plain in-order addition; lane L forms its own prefix
+            path = kPathChunkPrefix;
             const float wl = in ? w : 0.f;
             my_before = v.weight;
 #pragma unroll
@@ -1861,6 +1902,7 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
             }
             w_end = __shfl_sync(0xffffffffu, fadd(my_before, wl), 31);
           } else {
+            path = kPathChunkSequential;
             for (int k = 0; k < cnt; ++k) {
               const float wk = __shfl_sync(0xffffffffu, w, k);
               if (lane == k) my_before = w_end;
@@ -1881,7 +1923,9 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
         }
         if (fast) {
           v.weight = w_end;
+          count(path);
         } else {
+          count(kPathChunkExact);
           const uint32_t col = in ? rec_col[j0 + 32ull * g + lane] : 0u;
           for (int k = 0; k < cnt; ++k) {
             apply_update(v, __shfl_sync(0xffffffffu, sdf, k), __shfl_sync(0xffffffffu, w, k),
@@ -1901,7 +1945,6 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
   __shared__ float s_w[kApplyWarps][kApplyTile];
   __shared__ uint32_t s_col[kApplyWarps][kApplyTile];
   __shared__ uint8_t s_head[kApplyWarps][kApplyTile];
-  const int wb = threadIdx.x >> 5;
   const uint32_t n_tiles = (uint32_t)((total + kApplyTile - 1) / kApplyTile);
   for (;;) {
     uint32_t t = 0;
@@ -1939,11 +1982,13 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
       const uint32_t key = s_key[wb][o];
       const VoxelRef vr = locate_voxel(P, tab, key);
       if (vr.ptr == nullptr) continue;
+      ++n_short;
       TsdfVoxel v = *vr.ptr;
       int k = o;
       for (; k < kApplyTile && s_key[wb][k] == key; ++k) apply_update(v, s_sdf[wb][k], s_w[wb][k], s_col[wb][k], P.up);
       if (k == kApplyTile) {
         // a run that crosses the tile's end continues from global memory
+        ++n_crossed;
         for (unsigned long long j = base + kApplyTile; j < total && keys[j] == key; ++j) {
           apply_update(v, rec_sdf[j], rec_w[j], rec_col[j], P.up);
         }
@@ -1951,6 +1996,16 @@ k_apply(const ScanArgs* __restrict__ A, Tables tab, RecordView rv, LongRuns lr, 
       *vr.ptr = v;
     }
     __syncwarp();  // the staging arrays are reused by the warp's next tile
+  }
+  if (counting) {
+    n_short = __reduce_add_sync(0xffffffffu, n_short);
+    n_crossed = __reduce_add_sync(0xffffffffu, n_crossed);
+    if (lane == 0) {
+      s_paths[wb][kPathShortRun] = n_short;
+      s_paths[wb][kPathShortCrossed] = n_crossed;
+    }
+    __syncwarp();
+    if (lane < kApplyPaths && s_paths[wb][lane]) atomicAdd(&st->apply_paths[lane], s_paths[wb][lane]);
   }
 }
 
@@ -2189,8 +2244,9 @@ static int front_half(vbx_ctx* c, const ScanParams& P, const uint32_t* order, Ma
   return VBX_OK;
 }
 
-// update-record sort + the apply kernels
-static int sort_and_apply(vbx_ctx* c, Marks& mk, uint64_t* launches) {
+// update-record sort + the apply kernels.  given: the records' values are ordinals into these arrays, not
+// ray ids (debug_apply)
+static int sort_and_apply(vbx_ctx* c, Marks& mk, uint64_t* launches, const GivenRecords* given = nullptr) {
   cudaStream_t s = c->stream;
   const vbx_ctx::Capture* cap = c->cap;
   RecordView rv;
@@ -2227,7 +2283,12 @@ static int sort_and_apply(vbx_ctx* c, Marks& mk, uint64_t* launches) {
   lr.keep = c->keep_bits;
   lr.cap = c->max_updates / 32 + 1;
   // everything of the apply that does not depend on the map, on the (pipelined: scan-private) sort stream
-  k_apply_prep<<<c->grid_sms * 8, 256, 0, s>>>(c->d_args, c->tab, rv, c->ray_a, c->ray_c, lr, c->d_state);
+  if (given) {
+    k_apply_prep<true><<<c->grid_sms * 8, 256, 0, s>>>(c->d_args, c->tab, rv, c->ray_a, c->ray_c, lr, c->d_state, *given);
+  } else {
+    k_apply_prep<false><<<c->grid_sms * 8, 256, 0, s>>>(c->d_args, c->tab, rv, c->ray_a, c->ray_c, lr, c->d_state,
+                                                        GivenRecords{});
+  }
   mk.mark(6);
   if (cap) {
     // pipelined submission: the apply kernel runs behind the previous scan's apply, so the next scan's
@@ -2273,6 +2334,7 @@ static void fill_args(const vbx_ctx* c, const ScanParams& P, const float* xyz, c
   a->n = P.n;
   a->n_scan = P.n + 1;
   a->nb_cur = (uint32_t)c->nb_cur;
+  a->count_paths = c->count_apply_paths ? 1u : 0u;
 }
 
 // The synchronous calls' argument block goes through hand-off set 0's page-locked copy: the host writes it
@@ -2476,6 +2538,7 @@ int integrate_device(vbx_ctx* c, int kind, const float q[4], const float t[3], c
   c->counters[6] = (kind == VBX_MERGED) ? c->h_state->n_valid_points
                                         : (uint64_t)c->h_state->n_rays + c->h_state->n_clear_rays;
   c->counters[7] = launches;
+  for (int i = 0; i < kApplyPaths; ++i) c->apply_paths[i] = c->h_state->apply_paths[i];
   return VBX_OK;
 }
 
@@ -2577,7 +2640,7 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
       if (kp.func == (void*)k_back_begin || kp.func == (void*)k_rays_emit_warp<uint64_t> ||
           kp.func == (void*)k_rays_emit<uint64_t> || kp.func == (void*)k_assign) {
         prio.priority = walk_prio;
-      } else if (kp.func == (void*)k_sort<uint32_t> || kp.func == (void*)k_apply_prep) {
+      } else if (kp.func == (void*)k_sort<uint32_t> || kp.func == (void*)k_apply_prep<false>) {
         prio.priority = sort_prio;
       } else if (kp.func == (void*)k_apply) {
         prio.priority = c->prio_hi;
@@ -2853,6 +2916,111 @@ int debug_sort(vbx_ctx* c, const void* keys, int key_bytes, uint32_t n, int key_
   VBX_CUDA(c, cudaStreamSynchronize(s));
   VBX_CUDA(c, cudaGetLastError());
   return VBX_OK;
+}
+
+// vbx_debug_apply: touched id i -> hash position of block i, the records' keys (touched id, voxel) and
+// ordinals, and what the record sort and k_apply_prep otherwise learn from k_assign and the offset scan.
+// A block that is not a TSDF block of the map sets *bad.
+__global__ void k_debug_apply_setup(Tables tab, const uint64_t* __restrict__ bkeys, uint32_t nb,
+                                    const uint32_t* __restrict__ rec_block, const uint32_t* __restrict__ rec_voxel,
+                                    unsigned long long n, int L, uint32_t* keys, uint32_t* vals, ScanState* st,
+                                    uint32_t* bad) {
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < nb) {
+    const uint32_t hp = find_block(tab, bkeys[i]);
+    const int32_t slot = hp == 0xffffffffu ? -1 : tab.hslot[hp];
+    if (slot < 0 || (tab.slot_updated[slot] & kSlotNoTsdf)) *bad = 1u;
+    tab.touched_list[i] = hp;
+  }
+  if (i < n) {
+    keys[i] = (rec_block[i] << (3 * L)) | rec_voxel[i];
+    vals[i] = (uint32_t)i;
+  }
+  if (i == 0) {
+    st->total_updates = n;
+    st->total_found = n;
+    st->rec_key_bits = 3u * (uint32_t)L + (uint32_t)(32 - __clz(nb));
+  }
+}
+
+// Runs the production record sort, k_apply_prep (on the given values) and k_apply over caller-given
+// update records of blocks already in the map.  Record r belongs to block idx3[rec_block[r]], voxel
+// rec_voxel[r]; its sdf and weight are the final ones updateTsdfVoxel uses (after drop-off and sparsity).
+// Records of one voxel are applied in the order given.  Block updated() bits are left alone.
+int debug_apply(vbx_ctx* c, const int32_t* idx3, uint32_t nb, uint64_t n, const uint32_t* rec_block,
+                const uint32_t* rec_voxel, const float* sdf, const float* w, const uint8_t* rgba, uint64_t paths[16]) {
+  cudaStream_t s = c->stream;
+  if (n > c->max_updates) return fail(c, VBX_E_INVALID, "debug_apply: more records than max_updates_per_pass");
+  if (nb > c->tab.touched_cap) return fail(c, VBX_E_INVALID, "debug_apply: too many blocks");
+  for (uint64_t r = 0; r < n; ++r) {
+    if (rec_block[r] >= nb) return fail(c, VBX_E_INVALID, "debug_apply: block ordinal out of range");
+    if (rec_voxel[r] >= c->vox_per_block) return fail(c, VBX_E_INVALID, "debug_apply: voxel index >= voxels_per_side^3");
+  }
+  std::vector<uint64_t> bkeys(nb);
+  for (uint32_t i = 0; i < nb; ++i) bkeys[i] = pack3(idx3[3 * i], idx3[3 * i + 1], idx3[3 * i + 2]);
+  {
+    // a block listed twice would give one voxel two runs under different keys, applied side by side
+    std::vector<uint64_t> sorted = bkeys;
+    std::sort(sorted.begin(), sorted.end());
+    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) {
+      return fail(c, VBX_E_INVALID, "debug_apply: a block is listed twice");
+    }
+  }
+  // scratch: block keys, the records' block / voxel, sdf, weight, colour, and the "not in the map" flag
+  const size_t n4 = (size_t)n * 4;
+  char* buf = nullptr;
+  const size_t bytes = (size_t)nb * 8 + 5 * n4 + 4;
+  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&buf), bytes));
+  uint64_t* d_bkeys = reinterpret_cast<uint64_t*>(buf);
+  uint32_t* d_block = reinterpret_cast<uint32_t*>(buf + (size_t)nb * 8);
+  uint32_t* d_voxel = d_block + n;
+  float* d_sdf = reinterpret_cast<float*>(d_voxel + n);
+  float* d_w = d_sdf + n;
+  uint32_t* d_col = reinterpret_cast<uint32_t*>(d_w + n);
+  uint32_t* d_bad = d_col + n;
+  auto run = [&]() -> int {
+    VBX_CUDA(c, cudaMemcpyAsync(d_bkeys, bkeys.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, s));
+    VBX_CUDA(c, cudaMemcpyAsync(d_block, rec_block, n4, cudaMemcpyHostToDevice, s));
+    VBX_CUDA(c, cudaMemcpyAsync(d_voxel, rec_voxel, n4, cudaMemcpyHostToDevice, s));
+    VBX_CUDA(c, cudaMemcpyAsync(d_sdf, sdf, n4, cudaMemcpyHostToDevice, s));
+    VBX_CUDA(c, cudaMemcpyAsync(d_w, w, n4, cudaMemcpyHostToDevice, s));
+    VBX_CUDA(c, cudaMemcpyAsync(d_col, rgba, n4, cudaMemcpyHostToDevice, s));
+    VBX_CUDA(c, cudaMemsetAsync(d_bad, 0, 4, s));
+    ScanParams P;
+    const float q[4] = {1.f, 0.f, 0.f, 0.f}, t[3] = {0.f, 0.f, 0.f};
+    fill_params(c, VBX_SIMPLE, q, t, 0, 0, P);
+    ScanArgs a;
+    fill_args(c, P, nullptr, nullptr, &a);
+    a.count_paths = 1u;
+    if (int rc = upload_args(c, a)) return rc;
+    VBX_CUDA(c, cudaMemsetAsync(c->d_state, 0, sizeof(ScanState), s));
+    VBX_CUDA(c, cudaMemsetAsync(c->sort_plan[1], 0, sizeof(SortPlan), s));  // (sort_and_apply expects it cleared)
+    const uint64_t m = std::max<uint64_t>(n, nb);
+    if (m) {
+      k_debug_apply_setup<<<grid_for(m, 256), 256, 0, s>>>(c->tab, d_bkeys, nb, d_block, d_voxel, n, c->L, c->ckeys[0],
+                                                           c->cvals[0], c->d_state, d_bad);
+    }
+    uint32_t bad = 0;
+    VBX_CUDA(c, cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
+    VBX_CUDA(c, cudaStreamSynchronize(s));
+    if (bad) return fail(c, VBX_E_INVALID, "debug_apply: a block is not in the TSDF layer");
+    Marks mk;
+    mk.c = c;
+    mk.s = s;
+    uint64_t launches = 0;
+    const GivenRecords given{d_sdf, d_w, d_col};
+    if (int rc = sort_and_apply(c, mk, &launches, &given)) return rc;
+    VBX_CUDA(c, cudaMemcpyAsync(c->h_state, c->d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+    VBX_CUDA(c, cudaStreamSynchronize(s));
+    VBX_CUDA(c, cudaGetLastError());
+    if (int rc = check_state_errors(c, c->h_state->error)) return rc;
+    for (int i = 0; i < 16; ++i) c->apply_paths[i] = i < kApplyPaths ? c->h_state->apply_paths[i] : 0;
+    if (paths) std::memcpy(paths, c->apply_paths, sizeof(c->apply_paths));
+    return VBX_OK;
+  };
+  const int rc = run();
+  cudaFree(buf);
+  return rc;
 }
 
 // exclusive prefix sum of n host uint32 through the engine's scan kernel
