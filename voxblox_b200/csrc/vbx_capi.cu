@@ -134,6 +134,7 @@ void select_set(vbx_ctx* c, int k) {
   c->ray_list = S.ray_list;
   c->head_list = S.head_list;
   c->tab.touched_list = S.touched_list;
+  c->blocks = S.blocks;
   c->cnt = S.cnt;
   c->off = S.off;
   c->d_state = S.d_state;
@@ -228,6 +229,29 @@ void free_order_scratch(OrderScratch* g, uint32_t* big_list, uint32_t* first_bit
     if (p) cudaFree(p);
   }
   std::memset(g, 0, sizeof(*g));
+}
+
+// a hand-off set's private block table (vbx_engine.h, ScanBlocks): zeroed here, once; afterwards every call
+// clears the positions it used
+int alloc_scan_blocks(vbx_ctx* c, ScanBlocks* b) {
+  std::memset(b, 0, sizeof(*b));
+  b->cap = c->tab.touched_cap;
+  uint32_t size = 1;
+  while (size < 2 * b->cap) size <<= 1;
+  b->mask = size - 1;
+  VBX_CUDA(c, dmalloc(&b->table, size));
+  VBX_CUDA(c, dmalloc(&b->keys, b->cap));
+  VBX_CUDA(c, dmalloc(&b->pos, b->cap));
+  VBX_CUDA(c, cudaMemsetAsync(b->table, 0, (size_t)size * sizeof(uint32_t), c->stream_main));
+  VBX_CUDA(c, cudaStreamSynchronize(c->stream_main));
+  return VBX_OK;
+}
+void free_scan_blocks(ScanBlocks* b) {
+  void* ptrs[] = {b->table, b->keys, b->pos};
+  for (void* p : ptrs) {
+    if (p) cudaFree(p);
+  }
+  std::memset(b, 0, sizeof(*b));
 }
 
 }  // namespace vbx
@@ -410,6 +434,8 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
     a.ray_list = c->ray_list;
     a.head_list = c->head_list;
     a.touched_list = c->tab.touched_list;
+    if (int rc = alloc_scan_blocks(c, &a.blocks)) return rc;
+    c->blocks = a.blocks;
     a.cnt = c->cnt;
     a.off = c->off;
     a.d_state = c->d_state;
@@ -503,6 +529,7 @@ int ensure_async(vbx_ctx* c) {
     CK(dmalloc(&S.ray_list, np));
     CK(dmalloc(&S.head_list, np));
     CK(dmalloc(&S.touched_list, c->tab.touched_cap));
+    if (int rc = alloc_scan_blocks(c, &S.blocks)) return rc;
     CK(dmalloc(&S.cnt, np + 1));
     CK(dmalloc(&S.off, np + 1));
     CK(dmalloc(&S.d_state, 1));
@@ -565,6 +592,7 @@ void vbx_destroy(vbx_ctx* c) {
   if (c->mirror_slots) cudaFree(c->mirror_slots);
   for (int k = 0; k < vbx_ctx::kSets; ++k) {
     vbx_ctx::ScratchSet& S = c->set[k];
+    free_scan_blocks(&S.blocks);
     if (k > 0) {
       void* sp[] = {S.ray_p, S.ray_a, S.ray_c, S.ray_list, S.head_list, S.touched_list, S.cnt, S.off, S.d_state, S.d_xyz, S.d_rgba, S.pkeys0,
                     S.ckeys[0], S.ckeys[1], S.cvals[0], S.cvals[1], S.long_list, S.long_end, S.keep_bits,

@@ -111,7 +111,8 @@ struct ScanState {
   uint32_t esdf_ticket[6];   // ESDF queue kernels: work hand-out counters, rotating like the queue counters ([0..2] raise, [3..5] lower)
   uint32_t tile_ticket;      // k_apply: record tiles of the short runs handed out
   uint32_t apply_paths[12];  // k_apply: how often each arithmetic path ran, summed over the call (ApplyPath)
-  uint32_t reserved[2];
+  uint32_t ids_resolved;     // Merged: local block ids k_assign has resolved so far in this call (all passes)
+  uint32_t reserved;
 };
 static_assert(sizeof(ScanState) == 256, "the status block the host reads back is 256 bytes");
 static_assert(sizeof(ScanState::apply_paths) / 4 == kApplyPaths, "one word per apply path");
@@ -134,6 +135,19 @@ struct Tables {
   uint8_t* slot_has_esdf;      // [max_blocks] 1 once the ESDF layer holds this block
   TsdfVoxel* tsdf;        // [max_blocks << 3L]
   EsdfVoxel* esdf;        // [max_blocks << 3L] (allocated by vbx_esdf_create)
+};
+
+// A Merged scan's private block table (hand-off set private, beside touched_list).  The ray trace runs in
+// the front half, beside other scans' map-touching stages, so it must not read the block hash: it gives the
+// blocks it meets dense local ids here instead, and k_assign (walk stage, submission order) resolves each
+// id against the hash.  Open addressing keyed by pack3(block), value = local id + 1 (0: free).  The table is
+// zeroed once when it is allocated; k_assign clears the positions a call used.
+struct ScanBlocks {
+  uint32_t* table;            // [mask + 1], a power of two >= 2 * cap
+  unsigned long long* keys;   // [cap] local id -> packed block index (0: an id lost to a race, a hole)
+  uint32_t* pos;              // [cap] local id -> its table position
+  uint32_t mask;
+  uint32_t cap;               // = Tables::touched_cap
 };
 
 __host__ __device__ inline uint64_t pack3(int x, int y, int z) {
@@ -176,6 +190,7 @@ struct vbx_ctx {
   uint32_t hcap = 0;
   unsigned int grid_sms = 132;  // persistent-kernel grids are multiples of this (the device's SM count, queried at create; VBX_GRID_SMS overrides: tuning aid)
   vbx::Tables tab;
+  vbx::ScanBlocks blocks{};  // the current hand-off set's private block table
   // scratch
   uint32_t max_points = 0;
   uint64_t max_updates = 0;
@@ -226,8 +241,8 @@ struct vbx_ctx {
   uint32_t* d_nblocks = nullptr;      // [2] device copy, ping-pong: k_assign reads [nb_cur], writes [nb_cur ^ 1]
   int nb_cur = 0;
   // Asynchronous submission (vbx_tsdf_integrate_async): a scan passes through four stages -- front half
-  // (keys, bundle sort, bundle fold, offsets; does not touch the map) on one of kLanes front lanes, ray
-  // walk + block creation, record sort, apply -- so up to kSets scans are in flight, each owning one set
+  // (keys, bundle sort, bundle fold, offsets, Merged's ray trace; does not touch the map) on one of kLanes
+  // front lanes, block creation, record sort, apply -- so up to kSets scans are in flight, each owning one set
   // of hand-off buffers.  Map-touching stages run in submission order.  Each scan is one launch of a CUDA
   // graph per (hand-off set, front lane, kind), captured before its first use.  Set 0 / lane 0 are the
   // buffers the synchronous calls use; the others are allocated on the first asynchronous submission.
@@ -252,7 +267,8 @@ struct vbx_ctx {
     uint2* ray_c = nullptr;
     uint32_t* ray_list = nullptr;
     uint32_t* head_list = nullptr;   // bundle id -> sorted position of its head (read again by the ray walk)
-    uint32_t* touched_list = nullptr;  // touched id -> hash position (written by the walk, read by the apply)
+    uint32_t* touched_list = nullptr;  // touched id -> hash position (written by k_assign / the walk, read by the apply)
+    vbx::ScanBlocks blocks{};          // Merged: local block ids of the trace (written by the front half, read by k_assign)
     uint32_t* cnt = nullptr;
     uint32_t* off = nullptr;
     vbx::ScanState* d_state = nullptr;
@@ -303,7 +319,7 @@ struct vbx_ctx {
   bool async_ready = false;
   int prio_lo = 0, prio_hi = 0;  // stream priority range of the device
   // the streams a scan's graph is captured from (besides the front lane's and the main stream)
-  cudaStream_t stream_e = nullptr;  // ray walk + block creation
+  cudaStream_t stream_e = nullptr;  // block creation: k_back_begin, k_assign (Simple: and its ray walk)
   cudaStream_t stream_s = nullptr;  // record sort + apply preparation
   // non-null while a scan's graph is captured: the back half's streams and hand-off events (integrate_async)
   struct Capture {
@@ -407,6 +423,8 @@ int drain_async(vbx_ctx* c);           // wait for every asynchronously submitte
 int set_n_blocks(vbx_ctx* c, uint32_t n);
 int alloc_order_scratch(vbx_ctx* c, vbx::OrderScratch* g, uint32_t** big_list, uint32_t** first_bits);
 void free_order_scratch(vbx::OrderScratch* g, uint32_t* big_list, uint32_t* first_bits);
+int alloc_scan_blocks(vbx_ctx* c, vbx::ScanBlocks* b);  // a hand-off set's private block table, zeroed
+void free_scan_blocks(vbx::ScanBlocks* b);
 int init_bundle_order(vbx_ctx* c);     // rehash schedule + shared-memory opt-in of k_bundle_order
 int rebuild_hash(vbx_ctx* c);          // block hash rebuilt from slot_key (after removals / a pool overflow)
 void harvest_async(vbx_ctx* c, vbx_ctx::ScratchSet& S);  // collect a finished asynchronous scan's results

@@ -12,8 +12,12 @@
 //   k_rays_count     one thread per ray: DDA walk (RayCaster) that creates missing
 //                    blocks in the device hash and counts the voxels it will update
 //                    (allocateStorageAndGetVoxelPtr cc:91-134)
-//   scan + k_assign  offsets of every ray's update records; pool slots for new blocks
-//   k_rays_emit      second DDA walk writing (voxel id, ray id) records
+//   scan             offsets of every ray's update records
+//   k_rays_emit      DDA walk writing (block id, voxel) -> ray records; Merged: a warp per
+//                    ray (k_rays_emit_warp) at the end of the front half, keyed by local
+//                    block ids of a scan-private table, without reading the map
+//   k_assign         blocks found or created in the hash (Merged: the scan's local ids,
+//                    in submission order); pool slots for new blocks
 //   sort             stable radix sort by voxel id: every voxel's updates become one
 //                    run, ordered by ray rank
 //   k_apply_prep     per sorted record: sdf, weight, colour and a keep bit; the list
@@ -1228,17 +1232,81 @@ __global__ void k_back_begin(ScanState* st, uint32_t* hold) {
   }
 }
 
-// After the last walk that can create blocks: pool slots for the blocks created by this call
-// (updateLayerWithStoredBlocks, cc:137-147); a new block is born with all updated bits set (cc:128).
-__global__ void k_assign(Tables tab, const ScanArgs* __restrict__ A, uint32_t* __restrict__ nb, SortPlan* record_plan,
-                         ScanState* st) {
+// The walk stage's own work, in submission order: one thread block.
+//   Merged (single walk): the trace (front half) gave every block it met a local id in the scan's private
+//   table; here each id listed since the last pass finds or creates its block in the hash
+//   (allocateStorageAndGetVoxelPtr's find-or-emplace, cc:109-124), becomes the touched id the apply
+//   resolves, and marks an existing block updated (cc:128).  The call's last pass clears the table.
+//   Then, all integrators: pool slots for the blocks created by this call (updateLayerWithStoredBlocks,
+//   cc:137-147); a new block is born with all updated bits set (cc:128).
+constexpr int kAssignThreads = 512;
+__global__ void __launch_bounds__(kAssignThreads)
+k_assign(Tables tab, ScanBlocks sb, const ScanArgs* __restrict__ A, uint32_t* __restrict__ nb, SortPlan* record_plan,
+         ScanState* st) {
   const uint32_t* __restrict__ nb_in = nb + A->nb_cur;
   uint32_t* __restrict__ nb_out = nb + (A->nb_cur ^ 1u);
-  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j < (uint32_t)(sizeof(SortPlan) / 4)) reinterpret_cast<uint32_t*>(record_plan)[j] = 0u;  // for the record sort that follows
+  const uint32_t t = threadIdx.x;
+  for (uint32_t j = t; j < (uint32_t)(sizeof(SortPlan) / 4); j += blockDim.x) {
+    reinterpret_cast<uint32_t*>(record_plan)[j] = 0u;  // for the record sort that follows
+  }
+  const bool local_ids = A->P.kind == VBX_MERGED && A->P.single_walk;
+  const uint32_t n_ids = min(st->n_touch_ids, sb.cap);
+  if (local_ids) {
+    // a scan skipped behind the hold flag creates nothing (the host redoes it); its table is still cleared
+    const bool create = !(st->error & kSkipped);
+    const bool last_pass = A->P.emit_hi >= st->n_ray_list;
+    if (create) {
+      // the blocks this call creates are listed (and take pool slots) in local-id order: a block-wide
+      // scan over each round of ids instead of a counter the threads race for
+      __shared__ uint32_t warp_new[kAssignThreads / 32];
+      const uint32_t lane = t & 31u, w = t >> 5;
+      uint32_t n_new = st->n_new;  // (0 in every pass: only this kernel creates Merged blocks)
+      uint32_t touched = 0;
+      for (uint32_t id0 = st->ids_resolved; id0 < n_ids; id0 += blockDim.x) {
+        const uint32_t id = id0 + t;
+        const uint64_t key = id < n_ids ? sb.keys[id] : 0ull;  // (0: a hole)
+        bool created = false;
+        uint32_t hp = 0xffffffffu;
+        if (key != 0ull) {
+          hp = find_or_insert_block(tab, key, &created, st);
+          tab.touched_list[id] = hp;
+          if (hp != 0xffffffffu) {
+            const int32_t slot = tab.hslot[hp];
+            if (slot >= 0) tab.slot_updated[slot] = kTouchedBits;  // (*last_block)->updated().set(), cc:128
+            ++touched;
+          }
+        }
+        const unsigned int ballot = __ballot_sync(0xffffffffu, created);
+        if (lane == 0) warp_new[w] = __popc(ballot);
+        __syncthreads();
+        uint32_t j = n_new + __popc(ballot & ((1u << lane) - 1u));
+        for (uint32_t v = 0; v < blockDim.x / 32; ++v) {
+          if (v < w) j += warp_new[v];
+          n_new += warp_new[v];
+        }
+        if (created) {
+          if (j < tab.max_blocks) {
+            tab.new_list[j] = hp;
+          } else {
+            atomicOr(&st->error, kErrPoolFull);
+          }
+        }
+        __syncthreads();  // (warp_new is reused by the next round)
+      }
+      if (touched) atomicAdd(&st->n_touched, touched);
+      if (t == 0) st->n_new = n_new;
+    }
+    if (last_pass) {
+      for (uint32_t id = t; id < n_ids; id += blockDim.x) {
+        if (sb.keys[id] != 0ull) sb.table[sb.pos[id]] = 0u;
+      }
+    }
+  }
+  __syncthreads();  // every new block is in new_list and counted in n_new
   const uint32_t n_blocks_before = *nb_in;
-  const uint32_t n_new = min(st->n_new, tab.max_blocks);
-  if (j < n_new) {
+  const uint32_t n_new_all = *reinterpret_cast<volatile uint32_t*>(&st->n_new);
+  const uint32_t n_new = min(n_new_all, tab.max_blocks);
+  for (uint32_t j = t; j < n_new; j += blockDim.x) {
     const uint32_t slot = n_blocks_before + j;
     if (slot < tab.max_blocks) {
       const uint32_t hp = tab.new_list[j];
@@ -1249,10 +1317,11 @@ __global__ void k_assign(Tables tab, const ScanArgs* __restrict__ A, uint32_t* _
       atomicOr(&st->error, kErrPoolFull);
     }
   }
-  if (j == 0) {
-    const uint32_t after = min(n_blocks_before + st->n_new, tab.max_blocks);
+  if (t == 0) {
+    const uint32_t after = min(n_blocks_before + n_new_all, tab.max_blocks);
     st->n_blocks = after;
     *nb_out = after;
+    if (local_ids) st->ids_resolved = n_ids;
     // what the record sort has to look at: voxel bits + the bits of the touched ids handed out
     uint32_t vb = 0;
     while ((tab.vox_per_block >> vb) > 1u) ++vb;
@@ -1260,11 +1329,52 @@ __global__ void k_assign(Tables tab, const ScanArgs* __restrict__ A, uint32_t* _
   }
 }
 
+// How a block-run head of a walk becomes the id its update records are keyed by.  in_range: the voxel passed
+// the +-2^20-block coordinate check.  Both return 0xffffffff when the block has no id (an error is raised).
+//   HashBlockIds  Simple, anti-grazing and Fast: the block hash itself -- find-or-create (single walk) or
+//                 find, then the call's touched id (touch_block), and the block is marked updated.
+//   ScanBlockIds  Merged single walk (the trace, front half): the scan's private table only; k_assign
+//                 creates the blocks and marks them later, in submission order.
+struct HashBlockIds {
+  const ScanParams& P;
+  const Tables& tab;
+  ScanState* st;
+  __device__ uint32_t operator()(int bx, int by, int bz, bool in_range) const {
+    uint32_t hp;
+    if (P.single_walk) {
+      // the only walk of this ray: allocateStorageAndGetVoxelPtr's find-or-create, cc:91-134
+      if (!in_range) {
+        atomicOr(&st->error, kErrCoordRange);
+        return 0xffffffffu;
+      }
+      hp = ensure_block(tab, pack3(bx, by, bz), st);
+    } else {
+      hp = find_block(tab, pack3(bx, by, bz));
+    }
+    if (hp == 0xffffffffu) return hp;
+    const uint32_t tid = touch_block(tab, hp, P.epoch, st);
+    const int32_t slot = tab.hslot[hp];
+    if (slot >= 0) tab.slot_updated[slot] = kTouchedBits;  // (*last_block)->updated().set(), cc:128
+    return tid;
+  }
+};
+struct ScanBlockIds {
+  const ScanBlocks& sb;
+  ScanState* st;
+  __device__ uint32_t operator()(int bx, int by, int bz, bool in_range) const {
+    if (!in_range) {
+      atomicOr(&st->error, kErrCoordRange);
+      return 0xffffffffu;
+    }
+    return scan_block_id(sb, pack3(bx, by, bz), st);
+  }
+};
+
 // One ray, walked sequentially by the calling thread: RayCaster's loop (integrator_utils.cc:106-125)
-// with allocateStorageAndGetVoxelPtr's find-or-create per block change (cc:91-134).
-template <typename KeyT>
-__device__ void emit_ray_sequential(const ScanParams& P, const Tables& tab, const KeyT* __restrict__ keys, uint32_t i,
-                                    uint32_t rank, uint32_t head_pos, const float4* __restrict__ ray_p,
+// with allocateStorageAndGetVoxelPtr's find-or-create per block change (cc:91-134), through block_id.
+template <typename KeyT, typename BlockIds>
+__device__ void emit_ray_sequential(const ScanParams& P, const BlockIds& block_id, const KeyT* __restrict__ keys,
+                                    uint32_t i, uint32_t rank, uint32_t head_pos, const float4* __restrict__ ray_p,
                                     const uint32_t* __restrict__ cnt,
                                     const uint32_t* __restrict__ off, uint32_t* __restrict__ ckeys,
                                     uint32_t* __restrict__ cvals, ScanState* st) {
@@ -1280,7 +1390,7 @@ __device__ void emit_ray_sequential(const ScanParams& P, const Tables& tab, cons
   const KeyT own = (P.kind == VBX_MERGED) ? keys[head_pos] : (KeyT)0;
   uint32_t emitted = 0;
   int lbx = INT_MIN, lby = INT_MIN, lbz = INT_MIN;
-  uint32_t hp = 0, tid = 0;
+  uint32_t tid = 0;
   const uint32_t base = off[rank] - P.emit_base;
   const int mask = (1 << P.L) - 1;
   const int lim = (kCoordBias - 1) << P.L;
@@ -1291,23 +1401,10 @@ __device__ void emit_ray_sequential(const ScanParams& P, const Tables& tab, cons
     const int bx = d.cx >> P.L, by = d.cy >> P.L, bz = d.cz >> P.L;
     if (bx != lbx || by != lby || bz != lbz) {
       if (!owns_block(P, bx, by, bz)) {
-        hp = kNotOwned;  // another rank's block: the record keeps its place and is skipped by the apply
-      } else if (P.single_walk) {
-        // the only walk of this ray: allocateStorageAndGetVoxelPtr's find-or-create, cc:91-134
-        if (d.cx < -lim || d.cx > lim || d.cy < -lim || d.cy > lim || d.cz < -lim || d.cz > lim) {
-          atomicOr(&st->error, kErrCoordRange);
-          hp = 0xffffffffu;
-        } else {
-          hp = ensure_block(tab, pack3(bx, by, bz), st);
-        }
+        tid = kNotOwned;  // another rank's block: the record keeps its place and is skipped by the apply
       } else {
-        hp = find_block(tab, pack3(bx, by, bz));
-      }
-      tid = hp;  // (the two sentinels pass through)
-      if (hp != 0xffffffffu && hp != kNotOwned) {
-        tid = touch_block(tab, hp, P.epoch, st);
-        const int32_t slot = tab.hslot[hp];
-        if (slot >= 0) tab.slot_updated[slot] = kTouchedBits;  // (*last_block)->updated().set(), cc:128
+        const bool in_range = !(d.cx < -lim || d.cx > lim || d.cy < -lim || d.cy > lim || d.cz < -lim || d.cz > lim);
+        tid = block_id(bx, by, bz, in_range);  // (0xffffffff passes through: the record is skipped)
       }
       lbx = bx;
       lby = by;
@@ -1342,19 +1439,22 @@ __global__ void k_rays_emit(const ScanArgs* __restrict__ A, Tables tab, const Ke
     i = t;
     if (i >= P.n) return;
   }
-  emit_ray_sequential<KeyT>(P, tab, keys, i, t, head_pos, ray_p, cnt, off, ckeys, cvals, st);
+  emit_ray_sequential<KeyT>(P, HashBlockIds{P, tab, st}, keys, i, t, head_pos, ray_p, cnt, off, ckeys, cvals, st);
 }
 
-// The same walk cast by a WARP per ray (single-walk modes of the Merged integrator: a few thousand
-// rays of 100-300 steps each, far too few threads for a thread-per-ray walk).  The walk is the
-// stable three-way merge of the per-axis boundary-crossing chains (vbx_math.cuh, dda_rank):
+// The same walk cast by a WARP per ray: the trace of the Merged integrator's single walk (a few
+// thousand rays of 100-300 steps each, far too few threads for a thread-per-ray walk).  It runs at the
+// end of the front half and does not touch the map (it takes no Tables): a block-run head takes its
+// block's local id from the scan's private table (ScanBlockIds), and k_assign resolves those ids
+// against the block hash in the walk stage.  The walk is the stable three-way merge of the per-axis
+// boundary-crossing chains (vbx_math.cuh, dda_rank):
 //   1. lanes 0-2 build the chains T_a(k+1) = RN(T_a(k) + dt_a) in shared memory -- the only
 //      sequential part, and plain additions;
 //   2. all lanes rank the chain elements (two binary searches each) and scatter the voxel each
 //      step reaches into a shared walk list;
 //   3. the walk list is turned into records 32 at a time: block changes are found by comparing
-//      neighbouring lanes, only the first lane of each block run does the hash find-or-create,
-//      and the records leave the warp coalesced.
+//      neighbouring lanes, only the first lane of each block run looks its block up, and the
+//      records leave the warp coalesced.
 // Bit-identical to the sequential walk (tests/dda_merge_check.cc proves the merge against
 // dda_advance on the host); rays the merge form does not cover (axis-parallel components,
 // non-finite increments, more than kChainCap crossings on an axis) are walked by lane 0.
@@ -1363,7 +1463,7 @@ constexpr int kWalkCap = 3 * kChainCap;
 
 template <typename KeyT>
 __global__ void __launch_bounds__(128)
-k_rays_emit_warp(const ScanArgs* __restrict__ A, Tables tab, const KeyT* __restrict__ keys, const uint32_t* __restrict__ ray_list,
+k_rays_emit_warp(const ScanArgs* __restrict__ A, ScanBlocks sb, const KeyT* __restrict__ keys, const uint32_t* __restrict__ ray_list,
                  const uint32_t* __restrict__ head_list, const float4* __restrict__ ray_p, const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ off,
                  uint32_t* __restrict__ ckeys, uint32_t* __restrict__ cvals, ScanState* st) {
   const ScanParams P = A->P;
@@ -1377,6 +1477,7 @@ k_rays_emit_warp(const ScanArgs* __restrict__ A, Tables tab, const KeyT* __restr
   if (st->total_updates == 0) return;  // (a failed / to-be-redone call emits nothing)
   const int mask = (1 << P.L) - 1;
   const int lim = (kCoordBias - 1) << P.L;
+  const ScanBlockIds block_id{sb, st};
   for (uint32_t b = warp; b < n_rays; b += n_warps) {
     const uint32_t i = ray_list[b];  // rank b in the reference's bundle order -> bundle id
     const uint32_t c = cnt[i];
@@ -1430,7 +1531,7 @@ k_rays_emit_warp(const ScanArgs* __restrict__ A, Tables tab, const KeyT* __restr
     }
     if (!merge_ok) {
       if (lane == 0) {
-        emit_ray_sequential<KeyT>(P, tab, keys, i, b, head_list[i] & ~kHeadBig, ray_p, cnt, off, ckeys, cvals, st);
+        emit_ray_sequential<KeyT>(P, block_id, keys, i, b, head_list[i] & ~kHeadBig, ray_p, cnt, off, ckeys, cvals, st);
       }
       __syncwarp();
       continue;
@@ -1455,21 +1556,14 @@ k_rays_emit_warp(const ScanArgs* __restrict__ A, Tables tab, const KeyT* __restr
         pbz = cbz;
       }
       const bool head = valid && (bx != pbx || by != pby || bz != pbz);
-      uint32_t hp = 0u;
+      uint32_t hp = 0u;  // the block's local id
       if (head) {
-        // the first step inside a block: allocateStorageAndGetVoxelPtr's find-or-create, cc:91-134
+        // the first step inside a block: allocateStorageAndGetVoxelPtr's find-or-create (cc:91-134) happens
+        // in k_assign; here the block gets its id in the scan's table
         if (!owns_block(P, bx, by, bz)) {
           hp = kNotOwned;
-        } else if (vx < -lim || vx > lim || vy < -lim || vy > lim || vz < -lim || vz > lim) {
-          atomicOr(&st->error, kErrCoordRange);
-          hp = 0xffffffffu;
         } else {
-          hp = ensure_block(tab, pack3(bx, by, bz), st);
-        }
-        if (hp != 0xffffffffu && hp != kNotOwned) {
-          const int32_t slot = tab.hslot[hp];
-          if (slot >= 0) tab.slot_updated[slot] = kTouchedBits;  // (*last_block)->updated().set(), cc:128
-          hp = touch_block(tab, hp, P.epoch, st);      // from here on: the block's touched id
+          hp = block_id(bx, by, bz, !(vx < -lim || vx > lim || vy < -lim || vy > lim || vz < -lim || vz > lim));
         }
       }
       const unsigned int heads = __ballot_sync(0xffffffffu, head);
@@ -2163,7 +2257,19 @@ static int launch_bundle_order(vbx_ctx* c, cudaStream_t so, uint32_t n, const Ke
   return VBX_OK;
 }
 
-// Stages up to and including k_assign: everything that decides WHICH voxels are updated.  The per-scan values
+// The Merged single walk writes its update records in the front half (k_rays_emit_warp against the scan's
+// private block table); every other walk creates blocks itself and runs in the back half.
+static bool traced_in_front(const ScanParams& P) { return P.kind == VBX_MERGED && P.single_walk; }
+
+template <typename KeyT>
+static void launch_trace(vbx_ctx* c, const KeyT* keys, cudaStream_t s) {
+  // a few thousand bundles of 100-300 steps: one warp per ray
+  k_rays_emit_warp<KeyT><<<c->grid_sms * 8, 128, 0, s>>>(c->d_args, c->blocks, keys, c->ray_list, c->head_list, c->ray_p,
+                                                         c->cnt, c->off, c->ckeys[0], c->cvals[0], c->d_state);
+}
+
+// Stages up to the record offsets (for the Merged single walk also the trace that writes the update records):
+// everything that decides WHICH voxels are updated.  The per-scan values
 // come from the argument block (c->d_args), and the grids are sized for max_points_per_scan -- surplus threads
 // exit at once -- so that one captured graph serves scans of any size (the point sort's grid, whose surplus
 // blocks would wait between passes, is set per scan instead: update_scan_graph).
@@ -2240,6 +2346,13 @@ static int front_half(vbx_ctx* c, const ScanParams& P, const uint32_t* order, Ma
   }
   mk.mark(3);
   *launches += 1;
+  if (traced_in_front(P)) {
+    // the Merged trace needs nothing of the map: it ends the front half, so the walk stage (submission
+    // order) is left with k_assign's block creation
+    launch_trace<KeyT>(c, keys, s);
+    mk.mark(5);
+    *launches += 1;
+  }
   *keys_out = keys;
   return VBX_OK;
 }
@@ -2306,24 +2419,26 @@ static int sort_and_apply(vbx_ctx* c, Marks& mk, uint64_t* launches, const Given
   return VBX_OK;
 }
 
+// emitted: the front half has already written this call's update records (traced_in_front, one pass); the
+// passes of apply_in_passes trace their own rank window here.
 template <typename KeyT>
-static int back_half(vbx_ctx* c, const ScanParams& P, const KeyT* keys, Marks& mk, uint64_t* launches) {
+static int back_half(vbx_ctx* c, const ScanParams& P, const KeyT* keys, bool emitted, Marks& mk, uint64_t* launches) {
   cudaStream_t s = c->stream;
-  if (P.kind == VBX_MERGED && P.single_walk) {
-    // a few thousand bundles of 100-300 steps: one warp per ray
-    k_rays_emit_warp<KeyT><<<c->grid_sms * 8, 128, 0, s>>>(c->d_args, c->tab, keys, c->ray_list, c->head_list, c->ray_p,
-                                                           c->cnt, c->off, c->ckeys[0], c->cvals[0], c->d_state);
-  } else {
-    k_rays_emit<KeyT><<<grid_for(c->max_points, 128), 128, 0, s>>>(c->d_args, c->tab, keys, c->ray_list, c->head_list,
-                                                                   c->ray_p, c->cnt, c->off, c->ckeys[0], c->cvals[0],
-                                                                   c->d_state);
+  if (!emitted) {
+    if (traced_in_front(P)) {
+      launch_trace<KeyT>(c, keys, s);
+    } else {
+      k_rays_emit<KeyT><<<grid_for(c->max_points, 128), 128, 0, s>>>(c->d_args, c->tab, keys, c->ray_list, c->head_list,
+                                                                     c->ray_p, c->cnt, c->off, c->ckeys[0], c->cvals[0],
+                                                                     c->d_state);
+    }
+    mk.mark(5);
+    *launches += 1;
   }
-  mk.mark(5);
-  k_assign<<<grid_for(std::max<uint32_t>(c->tab.max_blocks, 1024), 256), 256, 0, s>>>(c->tab, c->d_args, c->d_nblocks,
-                                                                                      c->sort_plan[1], c->d_state);
+  k_assign<<<1, kAssignThreads, 0, s>>>(c->tab, c->blocks, c->d_args, c->d_nblocks, c->sort_plan[1], c->d_state);
   c->nb_cur ^= 1;
   mk.mark(4);
-  *launches += 2;
+  *launches += 1;
   return sort_and_apply(c, mk, launches);
 }
 
@@ -2364,8 +2479,10 @@ static int apply_in_passes(vbx_ctx* c, ScanArgs a, const KeyT* keys, Marks& mk, 
     const uint32_t nr = std::min(c->h_state->n_ray_list, n);
     for (uint32_t i = nr + 1; i < n; ++i) off[i] = off[n];
   }
-  uint32_t lo = 0, passes = 0;
-  while (lo < n) {
+  // every pass's slot range first: a call that cannot be split is refused before any pass runs (the Merged
+  // passes share the scan's block table, which only a call's last pass clears)
+  std::vector<std::pair<uint32_t, uint32_t>> ranges;
+  for (uint32_t lo = 0; lo < n;) {
     // the longest slot range starting at lo whose records fit
     const uint64_t room = (uint64_t)off[lo] + c->max_updates;
     uint32_t hi = (uint32_t)(std::upper_bound(off.begin() + lo, off.end(), room,
@@ -2373,20 +2490,23 @@ static int apply_in_passes(vbx_ctx* c, ScanArgs a, const KeyT* keys, Marks& mk, 
                              off.begin());
     hi = hi > 0 ? hi - 1 : 0;  // off[hi] <= room
     if (hi <= lo) return fail(c, VBX_E_CAPACITY, "a single ray has more updates than max_updates_per_pass");
-    const unsigned long long kp = (unsigned long long)off[hi] - off[lo];
-    if (kp > 0) {
-      a.P.emit_lo = lo;
-      a.P.emit_hi = hi;
-      a.P.emit_base = off[lo];
-      a.nb_cur = (uint32_t)c->nb_cur;
-      VBX_CUDA(c, cudaStreamSynchronize(s));  // (the previous pass has read its arguments)
-      if (int rc = upload_args(c, a)) return rc;
-      k_pass_begin<<<1, 1, 0, s>>>(c->d_state, kp);
-      *launches += 1;
-      if (int rc = back_half<KeyT>(c, a.P, keys, mk, launches)) return rc;
-      ++passes;
-    }
+    if (off[hi] > off[lo]) ranges.emplace_back(lo, hi);
     lo = hi;
+  }
+  uint32_t passes = 0;
+  for (const auto& r : ranges) {
+    const uint32_t lo = r.first, hi = r.second;
+    const unsigned long long kp = (unsigned long long)off[hi] - off[lo];
+    a.P.emit_lo = lo;
+    a.P.emit_hi = hi;  // (the last range ends at n: its k_assign clears the Merged block table)
+    a.P.emit_base = off[lo];
+    a.nb_cur = (uint32_t)c->nb_cur;
+    VBX_CUDA(c, cudaStreamSynchronize(s));  // (the previous pass has read its arguments)
+    if (int rc = upload_args(c, a)) return rc;
+    k_pass_begin<<<1, 1, 0, s>>>(c->d_state, kp);
+    *launches += 1;
+    if (int rc = back_half<KeyT>(c, a.P, keys, /*emitted=*/false, mk, launches)) return rc;
+    ++passes;
   }
   c->last_passes = passes;
   return VBX_OK;
@@ -2495,7 +2615,7 @@ int integrate_device(vbx_ctx* c, int kind, const float q[4], const float t[3], c
   if (int rc = front_half<uint64_t>(c, P, order, mk, &launches, &keys64)) return rc;
   {
     // own sort: K stays on the device, the whole call is enqueued without a host round trip
-    if (int rc = back_half<uint64_t>(c, P, keys64, mk, &launches)) return rc;
+    if (int rc = back_half<uint64_t>(c, P, keys64, traced_in_front(P), mk, &launches)) return rc;
     VBX_CUDA(c, cudaEventRecord(c->ev1, s));
     VBX_CUDA(c, cudaMemcpyAsync(c->h_state, c->d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
     VBX_CUDA(c, cudaStreamSynchronize(s));
@@ -2545,9 +2665,11 @@ int integrate_device(vbx_ctx* c, int kind, const float q[4], const float t[3], c
 // ------------------------------------------------------------- asynchronous submission
 // integratePointCloud without the host round trip: the call enqueues the scan and returns.  A scan
 // passes through four stages:
-//   front   keys, bundle sort, bundle fold, record offsets -- touches nothing of the map; the front
-//           lanes alternate, so several front halves can run side by side
-//   walk    ray walk with block creation, slot assignment
+//   front   keys, bundle sort, bundle fold, record offsets, and for Merged the ray trace that writes the
+//           update records against the scan's private block table -- touches nothing of the map; the
+//           front lanes alternate, so several front halves can run side by side
+//   walk    block creation (Merged: k_assign resolves the trace's local ids; Simple: the ray walk),
+//           slot assignment
 //   sort    record sort and apply preparation on scan-private buffers
 //   apply   the per-voxel updates
 // Stages that touch the map run in submission order (the walk of scan i+1 only inserts new hash
@@ -2601,7 +2723,7 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
     // synchronously, in order, from the retained inputs (recover_async, vbx_capi.cu).
     k_back_begin<<<1, 1, 0, c->stream_e>>>(S.d_state, c->d_hold);
     launches += 1;
-    if (int rc = back_half<uint64_t>(c, P, keys64, mk, &launches)) return rc;
+    if (int rc = back_half<uint64_t>(c, P, keys64, traced_in_front(P), mk, &launches)) return rc;
     VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, cap.apply));
     // every stream of the capture joins its origin
     const cudaStream_t joined[4] = {F.stream, c->stream_e, c->stream_s, c->stream_main};
@@ -2637,8 +2759,8 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
       }
       cudaLaunchAttributeValue prio = {};
       prio.priority = c->prio_lo;
-      if (kp.func == (void*)k_back_begin || kp.func == (void*)k_rays_emit_warp<uint64_t> ||
-          kp.func == (void*)k_rays_emit<uint64_t> || kp.func == (void*)k_assign) {
+      // (the Merged trace, k_rays_emit_warp, is a front-half node: it keeps the front priority)
+      if (kp.func == (void*)k_back_begin || kp.func == (void*)k_rays_emit<uint64_t> || kp.func == (void*)k_assign) {
         prio.priority = walk_prio;
       } else if (kp.func == (void*)k_sort<uint32_t> || kp.func == (void*)k_apply_prep<false>) {
         prio.priority = sort_prio;
