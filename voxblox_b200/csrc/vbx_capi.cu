@@ -11,8 +11,6 @@
 
 namespace vbx {
 
-int integrate_device(vbx_ctx* c, int kind, const float q[4], const float t[3], const float* d_xyz,
-                     const uint8_t* d_rgba, uint64_t n, int freespace);
 int debug_sort(vbx_ctx* c, const void* keys, int key_bytes, uint32_t n, int key_bits, void* keys_out,
                uint32_t* vals_out);
 int debug_scan(vbx_ctx* c, const uint32_t* in, uint32_t n, uint32_t* out);
@@ -23,8 +21,8 @@ int upload_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, const 
                   const uint8_t* updated_bits, int serialized);
 int remove_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m);
 int clear_layer(vbx_ctx* c, int layer);
-int integrate_async(vbx_ctx* c, int kind, const float q[4], const float t[3], const float* xyz, const uint8_t* rgba,
-                    uint64_t n, int freespace, int on_device);
+int integrate_async(vbx_ctx* c, const ScanRoute& sync, int kind, const float q[4], const float t[3], const float* xyz,
+                    const uint8_t* rgba, uint64_t n, int freespace, int on_device);
 int esdf_create(vbx_ctx* c, const vbx_esdf_config* cfg);
 int esdf_update(vbx_ctx* c, int batch, int clear_updated_flag);
 int esdf_update_blocks(vbx_ctx* c, const int32_t* idx3, uint64_t m, int incremental);
@@ -57,8 +55,8 @@ int refresh_host_mirror(vbx_ctx* c) {
 int set_n_blocks(vbx_ctx* c, uint32_t n) {
   c->n_blocks = n;
   VBX_CUDA(c, cudaMemcpyAsync(c->d_nblocks + c->nb_cur, &c->n_blocks, sizeof(uint32_t), cudaMemcpyHostToDevice,
-                              c->stream_main));
-  VBX_CUDA(c, cudaStreamSynchronize(c->stream_main));
+                              c->stream));
+  VBX_CUDA(c, cudaStreamSynchronize(c->stream));
   return VBX_OK;
 }
 
@@ -98,7 +96,8 @@ void harvest_async(vbx_ctx* c, vbx_ctx::ScratchSet& S) {
 
 // Every queued scan has been waited for.  Scans that could not be applied asynchronously (and the
 // scans queued behind them, which skipped their back halves) are redone synchronously from their
-// retained inputs, in submission order -- no scan is lost and the update order is the callers'.
+// retained inputs, in submission order -- no scan is lost and the update order is the callers'.  The redo
+// runs on hand-off set 0's scratch and only reads set k's input cloud.
 static int recover_async(vbx_ctx* c) {
   if (c->hash_dirty) {
     c->hash_dirty = false;
@@ -110,12 +109,12 @@ static int recover_async(vbx_ctx* c) {
   }
   if (todo.empty()) return VBX_OK;
   std::sort(todo.begin(), todo.end(), [](const vbx_ctx::ScratchSet* a, const vbx_ctx::ScratchSet* b) { return a->seq < b->seq; });
-  VBX_CUDA(c, cudaMemsetAsync(c->d_hold, 0, sizeof(uint32_t), c->stream_main));
+  VBX_CUDA(c, cudaMemsetAsync(c->d_hold, 0, sizeof(uint32_t), c->stream));
   int first_rc = VBX_OK;
   std::string first_msg;
   for (vbx_ctx::ScratchSet* S : todo) {
     S->redo = false;
-    const int rc = integrate_device(c, S->kind, S->q, S->t, S->in_xyz, S->in_rgba, S->n, S->freespace);
+    const int rc = integrate_device(c, sync_route(c), S->kind, S->q, S->t, S->in_xyz, S->in_rgba, S->n, S->freespace);
     c->async_redone += 1;
     if (rc != VBX_OK && first_rc == VBX_OK) {
       first_rc = rc;
@@ -126,51 +125,6 @@ static int recover_async(vbx_ctx* c) {
   return first_rc;
 }
 
-void select_set(vbx_ctx* c, int k) {
-  const vbx_ctx::ScratchSet& S = c->set[k];
-  c->ray_p = S.ray_p;
-  c->ray_a = S.ray_a;
-  c->ray_c = S.ray_c;
-  c->ray_list = S.ray_list;
-  c->head_list = S.head_list;
-  c->tab.touched_list = S.touched_list;
-  c->blocks = S.blocks;
-  c->cnt = S.cnt;
-  c->off = S.off;
-  c->d_state = S.d_state;
-  c->h_state = S.h_state;
-  c->d_args = S.d_args;
-  c->h_args = S.h_args;
-  c->d_xyz = S.d_xyz;
-  c->d_rgba = S.d_rgba;
-  c->pkeys[0] = S.pkeys0;
-  for (int i = 0; i < 2; ++i) {
-    c->ckeys[i] = S.ckeys[i];
-    c->cvals[i] = S.cvals[i];
-  }
-  c->long_list = S.long_list;
-  c->long_end = S.long_end;
-  c->keep_bits = S.keep_bits;
-  c->sort_plan[1] = S.sort_plan1;
-  c->sort_status[1] = S.sort_status1;
-}
-
-void select_lane(vbx_ctx* c, int l) {
-  const vbx_ctx::FrontLane& F = c->lane[l];
-  c->big_list = F.big_list;
-  c->first_bits = F.first_bits;
-  c->order_scratch = F.order_scratch;
-  c->side_stream = F.side;
-  c->ev_fork = F.ev_fork;
-  c->ev_join = F.ev_join;
-  c->pkeys[1] = F.pkeys1;
-  c->pvals[0] = F.pvals[0];
-  c->pvals[1] = F.pvals[1];
-  c->sort_plan[0] = F.sort_plan0;
-  c->sort_status[0] = F.sort_status0;
-  c->scan_status = F.scan_status;
-}
-
 int drain_async(vbx_ctx* c) {
   for (int k = 0; k < c->sets_in_use; ++k) {
     vbx_ctx::ScratchSet& S = c->set[(c->async_seq + k) % c->sets_in_use];  // oldest submission first
@@ -178,10 +132,6 @@ int drain_async(vbx_ctx* c) {
     VBX_CUDA(c, cudaEventSynchronize(S.back_done));
     harvest_async(c, S);
   }
-  // synchronous calls use hand-off set 0 and front lane 0 on the main stream
-  select_set(c, 0);
-  select_lane(c, 0);
-  c->stream = c->stream_main;
   if (int rc = recover_async(c)) {
     if (!c->deferred_rc) return rc;
   }
@@ -199,59 +149,118 @@ static cudaError_t dmalloc(T** p, size_t count) {
   return cudaMalloc(reinterpret_cast<void**>(p), count * sizeof(T));
 }
 
-// k_bundle_order's tables for one front lane (vbx_order.cuh)
-int alloc_order_scratch(vbx_ctx* c, OrderScratch* g, uint32_t** big_list, uint32_t** first_bits) {
-  const size_t np = c->max_points;
-  std::memset(g, 0, sizeof(*g));
-  g->cap = (uint32_t)np;
-  // the bucket count after np insertions
-  uint32_t buckets = 1;
-  for (int k = 0; k < c->rehash.count && c->rehash.m[k] < np; ++k) buckets = c->rehash.n[k];
-  g->bucket_cap = buckets;
-  VBX_CUDA(c, dmalloc(&g->h, 2 * np));
-  VBX_CUDA(c, dmalloc(&g->tau, np));
-  VBX_CUDA(c, dmalloc(&g->tau2, np));
-  VBX_CUDA(c, dmalloc(&g->next, np));
-  VBX_CUDA(c, dmalloc(&g->bkt, np));
-  VBX_CUDA(c, dmalloc(&g->A, np));
-  VBX_CUDA(c, dmalloc(&g->bhead, (size_t)buckets));
-  VBX_CUDA(c, dmalloc(&g->head_of, 2 * np));
-  VBX_CUDA(c, dmalloc(&g->wp, 2 * (np / 32 + 2)));
-  VBX_CUDA(c, dmalloc(&g->cta_tot, 64));
-  VBX_CUDA(c, dmalloc(big_list, np / 256 + 2));
-  VBX_CUDA(c, dmalloc(first_bits, 2 * (np / 32 + 2)));
-  VBX_CUDA(c, cudaMemsetAsync(*first_bits, 0, 2 * (np / 32 + 2) * sizeof(uint32_t), c->stream_main));
-  return VBX_OK;
-}
-void free_order_scratch(OrderScratch* g, uint32_t* big_list, uint32_t* first_bits) {
-  void* ptrs[] = {g->h, g->tau, g->tau2, g->next, g->bkt, g->A, g->bhead, g->head_of, g->wp, g->cta_tot, big_list, first_bits};
-  for (void* p : ptrs) {
-    if (p) cudaFree(p);
+// Everything a hand-off set owns except the pipeline's streams and events (ensure_async).  Its private block
+// table is zeroed here, once; afterwards every call clears the positions it used.
+static int alloc_set(vbx_ctx* c, vbx_ctx::ScratchSet& S) {
+  const size_t np = c->max_points, nu = c->max_updates;
+  VBX_CUDA(c, dmalloc(&S.ray_p, np));
+  VBX_CUDA(c, dmalloc(&S.ray_a, np));
+  VBX_CUDA(c, dmalloc(&S.ray_c, np));
+  VBX_CUDA(c, dmalloc(&S.ray_list, np));
+  VBX_CUDA(c, dmalloc(&S.head_list, np));
+  VBX_CUDA(c, dmalloc(&S.touched_list, c->tab.touched_cap));
+  VBX_CUDA(c, dmalloc(&S.cnt, np + 1));
+  VBX_CUDA(c, dmalloc(&S.off, np + 1));
+  VBX_CUDA(c, dmalloc(&S.d_state, 1));
+  VBX_CUDA(c, cudaMallocHost(reinterpret_cast<void**>(&S.h_state), sizeof(ScanState)));
+  if (int rc = alloc_scan_args(c, S)) return rc;
+  VBX_CUDA(c, dmalloc(&S.d_xyz, 3 * np));
+  VBX_CUDA(c, dmalloc(&S.d_rgba, 4 * np));
+  VBX_CUDA(c, dmalloc(&S.pkeys0, np));
+  for (int i = 0; i < 2; ++i) {
+    VBX_CUDA(c, dmalloc(&S.ckeys[i], nu));
+    VBX_CUDA(c, dmalloc(&S.cvals[i], nu));
   }
-  std::memset(g, 0, sizeof(*g));
+  VBX_CUDA(c, dmalloc(&S.long_list, nu / 32 + 1));
+  VBX_CUDA(c, dmalloc(&S.long_end, nu / 32 + 1));
+  VBX_CUDA(c, dmalloc(&S.keep_bits, nu / 32 + 1));
+  VBX_CUDA(c, dmalloc(&S.sort_plan1, 1));
+  VBX_CUDA(c, dmalloc(&S.sort_status1, (size_t)4 * c->sort_tiles_cap[1] * kRadix));
+  ScanBlocks& b = S.blocks;
+  b.cap = c->tab.touched_cap;
+  uint32_t size = 1;
+  while (size < 2 * b.cap) size <<= 1;
+  b.mask = size - 1;
+  VBX_CUDA(c, dmalloc(&b.table, size));
+  VBX_CUDA(c, dmalloc(&b.keys, b.cap));
+  VBX_CUDA(c, dmalloc(&b.pos, b.cap));
+  VBX_CUDA(c, cudaMemsetAsync(b.table, 0, (size_t)size * sizeof(uint32_t), c->stream));
+  VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), c->stream));
+  VBX_CUDA(c, cudaStreamSynchronize(c->stream));
+  return VBX_OK;
 }
 
-// a hand-off set's private block table (vbx_engine.h, ScanBlocks): zeroed here, once; afterwards every call
-// clears the positions it used
-int alloc_scan_blocks(vbx_ctx* c, ScanBlocks* b) {
-  std::memset(b, 0, sizeof(*b));
-  b->cap = c->tab.touched_cap;
-  uint32_t size = 1;
-  while (size < 2 * b->cap) size <<= 1;
-  b->mask = size - 1;
-  VBX_CUDA(c, dmalloc(&b->table, size));
-  VBX_CUDA(c, dmalloc(&b->keys, b->cap));
-  VBX_CUDA(c, dmalloc(&b->pos, b->cap));
-  VBX_CUDA(c, cudaMemsetAsync(b->table, 0, (size_t)size * sizeof(uint32_t), c->stream_main));
-  VBX_CUDA(c, cudaStreamSynchronize(c->stream_main));
-  return VBX_OK;
-}
-void free_scan_blocks(ScanBlocks* b) {
-  void* ptrs[] = {b->table, b->keys, b->pos};
-  for (void* p : ptrs) {
+static void free_set(vbx_ctx::ScratchSet& S) {
+  const ScanBlocks& b = S.blocks;
+  void* dev[] = {S.ray_p, S.ray_a, S.ray_c, S.ray_list, S.head_list, S.touched_list, b.table, b.keys, b.pos, S.cnt,
+                 S.off, S.d_state, S.d_args, S.d_xyz, S.d_rgba, S.pkeys0, S.ckeys[0], S.ckeys[1], S.cvals[0],
+                 S.cvals[1], S.long_list, S.long_end, S.keep_bits, S.sort_plan1, S.sort_status1};
+  for (void* p : dev) {
     if (p) cudaFree(p);
   }
-  std::memset(b, 0, sizeof(*b));
+  if (S.h_state) cudaFreeHost(S.h_state);
+  if (S.h_args) cudaFreeHost(S.h_args);
+  for (auto& per_lane : S.graph) {
+    for (vbx_ctx::ScanGraph& G : per_lane) {
+      if (G.exec) cudaGraphExecDestroy(G.exec);
+      if (G.graph) cudaGraphDestroy(G.graph);
+    }
+  }
+  if (S.stream) cudaStreamDestroy(S.stream);
+  for (cudaEvent_t e : {S.copy_done, S.walked, S.sorted, S.applied, S.back_done, S.front_start, S.front_done}) {
+    if (e) cudaEventDestroy(e);
+  }
+}
+
+// Everything a front lane owns except the pipeline's stream and event (ensure_async).
+static int alloc_lane(vbx_ctx* c, vbx_ctx::FrontLane& F) {
+  const size_t np = c->max_points;
+  VBX_CUDA(c, dmalloc(&F.pkeys1, np));
+  VBX_CUDA(c, dmalloc(&F.pvals[0], np));
+  VBX_CUDA(c, dmalloc(&F.pvals[1], np));
+  VBX_CUDA(c, dmalloc(&F.sort_plan0, 1));
+  VBX_CUDA(c, dmalloc(&F.sort_status0, (size_t)8 * c->sort_tiles_cap[0] * kRadix));
+  VBX_CUDA(c, dmalloc(&F.scan_status, (np + 1) / kScanTile + 4));
+  VBX_CUDA(c, dmalloc(&F.big_list, np / 256 + 2));
+  VBX_CUDA(c, dmalloc(&F.first_bits, 2 * (np / 32 + 2)));
+  VBX_CUDA(c, cudaMemsetAsync(F.first_bits, 0, 2 * (np / 32 + 2) * sizeof(uint32_t), c->stream));
+  // k_bundle_order's tables (vbx_order.cuh), for the bucket count after np insertions
+  OrderScratch& g = F.order_scratch;
+  g.cap = (uint32_t)np;
+  uint32_t buckets = 1;
+  for (int k = 0; k < c->rehash.count && c->rehash.m[k] < np; ++k) buckets = c->rehash.n[k];
+  g.bucket_cap = buckets;
+  VBX_CUDA(c, dmalloc(&g.h, 2 * np));
+  VBX_CUDA(c, dmalloc(&g.tau, np));
+  VBX_CUDA(c, dmalloc(&g.tau2, np));
+  VBX_CUDA(c, dmalloc(&g.next, np));
+  VBX_CUDA(c, dmalloc(&g.bkt, np));
+  VBX_CUDA(c, dmalloc(&g.A, np));
+  VBX_CUDA(c, dmalloc(&g.bhead, (size_t)buckets));
+  VBX_CUDA(c, dmalloc(&g.head_of, 2 * np));
+  VBX_CUDA(c, dmalloc(&g.wp, 2 * (np / 32 + 2)));
+  VBX_CUDA(c, dmalloc(&g.cta_tot, 64));
+  VBX_CUDA(c, cudaStreamCreateWithPriority(&F.side, cudaStreamNonBlocking, c->prio_lo));
+  VBX_CUDA(c, cudaEventCreateWithFlags(&F.ev_fork, cudaEventDisableTiming));
+  VBX_CUDA(c, cudaEventCreateWithFlags(&F.ev_join, cudaEventDisableTiming));
+  return VBX_OK;
+}
+
+static void free_lane(vbx_ctx::FrontLane& F) {
+  const OrderScratch& g = F.order_scratch;
+  void* dev[] = {F.pkeys1, F.pvals[0], F.pvals[1], F.sort_plan0, F.sort_status0, F.scan_status, F.big_list, F.first_bits,
+                 g.h, g.tau, g.tau2, g.next, g.bkt, g.A, g.bhead, g.head_of, g.wp, g.cta_tot};
+  for (void* p : dev) {
+    if (p) cudaFree(p);
+  }
+  if (F.side) {
+    cudaStreamSynchronize(F.side);
+    cudaStreamDestroy(F.side);
+  }
+  for (cudaEvent_t e : {F.ev_fork, F.ev_join, F.done}) {
+    if (e) cudaEventDestroy(e);
+  }
+  if (F.stream) cudaStreamDestroy(F.stream);
 }
 
 }  // namespace vbx
@@ -338,10 +347,9 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
   CK(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));  // numerically lower = higher priority
   c->prio_lo = prio_lo;
   c->prio_hi = prio_hi;
-  CK(cudaStreamCreateWithPriority(&c->stream_main, cudaStreamNonBlocking, prio_hi));
+  CK(cudaStreamCreateWithPriority(&c->stream, cudaStreamNonBlocking, prio_hi));
   CK(cudaStreamCreateWithFlags(&c->stream_c, cudaStreamNonBlocking));
   CK(cudaStreamCreateWithFlags(&c->stream_c2, cudaStreamNonBlocking));
-  c->stream = c->stream_main;
   CK(cudaEventCreate(&c->ev0));
   CK(cudaEventCreate(&c->ev1));
   CK(cudaEventCreate(&c->tev0));
@@ -361,7 +369,6 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
   // ids lost to first-touch races stay unused (vbx_hash.cuh); (id, voxel) must fit a 32-bit record key
   t.touched_cap = (uint32_t)std::min<uint64_t>((uint64_t)o.max_blocks + 65536u, (0xffffffffull >> (3 * c->L)) - 1);
   t.vox_per_block = c->vox_per_block;
-  CK(dmalloc(&t.touched_list, t.touched_cap));
   CK(dmalloc(&t.slot_key, o.max_blocks));
   CK(dmalloc(&t.slot_updated, o.max_blocks));
   CK(dmalloc(&t.slot_esdf_updated, o.max_blocks));
@@ -376,97 +383,22 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
   // new Block: voxels default-constructed = all zero bytes (core/voxel.h:12-16)
   CK(cudaMemsetAsync(t.tsdf, 0, (size_t)o.max_blocks * c->vox_per_block * sizeof(TsdfVoxel), c->stream));
   const size_t np = c->max_points;
-  CK(dmalloc(&c->d_xyz, 3 * np));
-  CK(dmalloc(&c->d_rgba, 4 * np));
-  for (int i = 0; i < 2; ++i) {
-    CK(dmalloc(&c->pkeys[i], np));
-    CK(dmalloc(&c->pvals[i], np));
-    CK(dmalloc(&c->ckeys[i], (size_t)c->max_updates));
-    CK(dmalloc(&c->cvals[i], (size_t)c->max_updates));
-  }
   CK(dmalloc(&c->order, np));
   CK(dmalloc(&c->order_inv, np));
-  CK(dmalloc(&c->ray_list, np));
   if (int rc = init_bundle_order(c)) return rc;
-  CK(dmalloc(&c->head_list, np));
-  if (int rc = alloc_order_scratch(c, &c->order_scratch, &c->big_list, &c->first_bits)) return rc;
-  for (int l = 0; l < vbx_ctx::kLanes; ++l) {
-    CK(cudaStreamCreateWithPriority(&c->lane[l].side, cudaStreamNonBlocking, prio_lo));
-    CK(cudaEventCreateWithFlags(&c->lane[l].ev_fork, cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&c->lane[l].ev_join, cudaEventDisableTiming));
-  }
-  CK(dmalloc(&c->long_list, (size_t)(c->max_updates / 32 + 1)));
-  CK(dmalloc(&c->long_end, (size_t)(c->max_updates / 32 + 1)));
-  CK(dmalloc(&c->keep_bits, (size_t)(c->max_updates / 32 + 1)));
-  CK(dmalloc(&c->ray_p, np));
-  CK(dmalloc(&c->ray_c, np));
-  CK(dmalloc(&c->ray_a, np));
-  CK(dmalloc(&c->cnt, np + 1));
-  CK(dmalloc(&c->off, np + 1));
-  {
-    // own sort / scan state
-    c->sort_tiles_cap[0] = (uint32_t)((np + kSortTile - 1) / kSortTile);
-    c->sort_tiles_cap[1] = (uint32_t)((c->max_updates + kSortTile - 1) / kSortTile);
-    for (int i = 0; i < 2; ++i) {
-      CK(dmalloc(&c->sort_plan[i], 1));
-      const size_t words = (size_t)(i == 0 ? 8 : 4) * c->sort_tiles_cap[i] * kRadix;
-      CK(dmalloc(&c->sort_status[i], words));
-    }
-    CK(dmalloc(&c->scan_status, (np + 1) / kScanTile + 4));
-  }
+  c->sort_tiles_cap[0] = (uint32_t)((np + kSortTile - 1) / kSortTile);
+  c->sort_tiles_cap[1] = (uint32_t)((c->max_updates + kSortTile - 1) / kSortTile);
   CK(dmalloc(&c->set_start, 1u << 20));
   CK(dmalloc(&c->set_observed, 1u << 20));
   CK(cudaMemsetAsync(c->set_start, 0, sizeof(unsigned long long) << 20, c->stream));
   CK(cudaMemsetAsync(c->set_observed, 0, sizeof(unsigned long long) << 20, c->stream));
-  CK(dmalloc(&c->d_state, 1));
-  CK(cudaMemsetAsync(c->d_state, 0, sizeof(ScanState), c->stream));
-  CK(cudaMallocHost(reinterpret_cast<void**>(&c->h_state), sizeof(ScanState)));
   CK(dmalloc(&c->d_nblocks, 2));
   CK(cudaMemsetAsync(c->d_nblocks, 0, 2 * sizeof(uint32_t), c->stream));
   CK(dmalloc(&c->d_hold, 1));
   CK(cudaMemsetAsync(c->d_hold, 0, sizeof(uint32_t), c->stream));
-  {
-    // hand-off set 0 / front lane 0 are the buffers above; the others are allocated by ensure_async
-    vbx_ctx::ScratchSet& a = c->set[0];
-    a.ray_p = c->ray_p;
-    a.ray_a = c->ray_a;
-    a.ray_c = c->ray_c;
-    a.ray_list = c->ray_list;
-    a.head_list = c->head_list;
-    a.touched_list = c->tab.touched_list;
-    if (int rc = alloc_scan_blocks(c, &a.blocks)) return rc;
-    c->blocks = a.blocks;
-    a.cnt = c->cnt;
-    a.off = c->off;
-    a.d_state = c->d_state;
-    a.h_state = c->h_state;
-    if (int rc = alloc_scan_args(c, a)) return rc;
-    c->d_args = a.d_args;
-    c->h_args = a.h_args;
-    a.d_xyz = c->d_xyz;
-    a.d_rgba = c->d_rgba;
-    a.pkeys0 = c->pkeys[0];
-    for (int i = 0; i < 2; ++i) {
-      a.ckeys[i] = c->ckeys[i];
-      a.cvals[i] = c->cvals[i];
-    }
-    a.long_list = c->long_list;
-    a.long_end = c->long_end;
-    a.keep_bits = c->keep_bits;
-    a.sort_plan1 = c->sort_plan[1];
-    a.sort_status1 = c->sort_status[1];
-    vbx_ctx::FrontLane& f = c->lane[0];
-    f.pkeys1 = c->pkeys[1];
-    f.pvals[0] = c->pvals[0];
-    f.pvals[1] = c->pvals[1];
-    f.sort_plan0 = c->sort_plan[0];
-    f.sort_status0 = c->sort_status[0];
-    f.scan_status = c->scan_status;
-    f.big_list = c->big_list;
-    f.first_bits = c->first_bits;
-    f.order_scratch = c->order_scratch;
-    select_lane(c, 0);
-  }
+  // the synchronous calls' scratch; ensure_async allocates the other sets and lanes
+  if (int rc = alloc_set(c, c->set[0])) return rc;
+  if (int rc = alloc_lane(c, c->lane[0])) return rc;
   CK(cudaStreamSynchronize(c->stream));
 #undef CK
   return VBX_OK;
@@ -485,7 +417,6 @@ int ensure_async(vbx_ctx* c) {
   } while (0)
   if (const char* e = std::getenv("VBX_ASYNC_SETS")) c->sets_in_use = std::max(2, std::min(std::atoi(e), (int)vbx_ctx::kSets));
   if (const char* e = std::getenv("VBX_ASYNC_LANES")) c->lanes_in_use = std::max(1, std::min(std::atoi(e), (int)vbx_ctx::kLanes));
-  const size_t np = c->max_points;
   CK(cudaStreamCreateWithPriority(&c->stream_e, cudaStreamNonBlocking, std::min(c->prio_lo, c->prio_hi + 1)));
   CK(cudaStreamCreateWithPriority(&c->stream_s, cudaStreamNonBlocking, std::min(c->prio_lo, c->prio_hi + 2)));
   for (cudaEvent_t& e : c->cap_ev) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -494,20 +425,14 @@ int ensure_async(vbx_ctx* c) {
     CK(cudaStreamCreateWithPriority(&F.stream, cudaStreamNonBlocking, c->prio_lo));
     CK(cudaEventCreateWithFlags(&F.done, cudaEventDisableTiming));
     if (l == 0) continue;
-    CK(dmalloc(&F.pkeys1, np));
-    CK(dmalloc(&F.pvals[0], np));
-    CK(dmalloc(&F.pvals[1], np));
-    CK(dmalloc(&F.sort_plan0, 1));
-    CK(dmalloc(&F.sort_status0, (size_t)8 * c->sort_tiles_cap[0] * kRadix));
-    CK(dmalloc(&F.scan_status, (np + 1) / kScanTile + 4));
-    if (int rc = alloc_order_scratch(c, &F.order_scratch, &F.big_list, &F.first_bits)) return rc;
+    if (int rc = alloc_lane(c, F)) return rc;
   }
   // diagnostic: with VBX_ASYNC_TIMELINE set the hand-off events keep timestamps (vbx_debug_async_timeline)
   c->timeline = std::getenv("VBX_ASYNC_TIMELINE") != nullptr;
   const unsigned int evf = c->timeline ? cudaEventDefault : cudaEventDisableTiming;
   if (c->timeline) {
     CK(cudaEventCreate(&c->timeline_ref));
-    CK(cudaEventRecord(c->timeline_ref, c->stream_main));
+    CK(cudaEventRecord(c->timeline_ref, c->stream));
   }
   for (int k = 0; k < c->sets_in_use; ++k) {
     vbx_ctx::ScratchSet& S = c->set[k];
@@ -522,30 +447,7 @@ int ensure_async(vbx_ctx* c) {
       CK(cudaEventCreate(&S.front_done));
     }
     if (k == 0) continue;
-    if (int rc = alloc_scan_args(c, S)) return rc;
-    CK(dmalloc(&S.ray_p, np));
-    CK(dmalloc(&S.ray_a, np));
-    CK(dmalloc(&S.ray_c, np));
-    CK(dmalloc(&S.ray_list, np));
-    CK(dmalloc(&S.head_list, np));
-    CK(dmalloc(&S.touched_list, c->tab.touched_cap));
-    if (int rc = alloc_scan_blocks(c, &S.blocks)) return rc;
-    CK(dmalloc(&S.cnt, np + 1));
-    CK(dmalloc(&S.off, np + 1));
-    CK(dmalloc(&S.d_state, 1));
-    CK(cudaMallocHost(reinterpret_cast<void**>(&S.h_state), sizeof(ScanState)));
-    CK(dmalloc(&S.d_xyz, 3 * np));
-    CK(dmalloc(&S.d_rgba, 4 * np));
-    CK(dmalloc(&S.pkeys0, np));
-    for (int i = 0; i < 2; ++i) {
-      CK(dmalloc(&S.ckeys[i], (size_t)c->max_updates));
-      CK(dmalloc(&S.cvals[i], (size_t)c->max_updates));
-    }
-    CK(dmalloc(&S.long_list, (size_t)(c->max_updates / 32 + 1)));
-    CK(dmalloc(&S.long_end, (size_t)(c->max_updates / 32 + 1)));
-    CK(dmalloc(&S.keep_bits, (size_t)(c->max_updates / 32 + 1)));
-    CK(dmalloc(&S.sort_plan1, 1));
-    CK(dmalloc(&S.sort_status1, (size_t)4 * c->sort_tiles_cap[1] * kRadix));
+    if (int rc = alloc_set(c, S)) return rc;
   }
 #undef CK
   c->async_ready = true;
@@ -558,7 +460,7 @@ extern "C" {
 void vbx_destroy(vbx_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
-  if (c->stream_main) cudaStreamSynchronize(c->stream_main);
+  if (c->stream) cudaStreamSynchronize(c->stream);
   if (c->stream_c) cudaStreamSynchronize(c->stream_c);
   if (c->stream_c2) cudaStreamSynchronize(c->stream_c2);
   for (int k = 0; k < vbx_ctx::kSets; ++k) {
@@ -567,76 +469,21 @@ void vbx_destroy(vbx_ctx* c) {
   for (int l = 0; l < vbx_ctx::kLanes; ++l) {
     if (c->lane[l].stream) cudaStreamSynchronize(c->lane[l].stream);
   }
-  // restore the aliases of hand-off set 0 / lane 0 before freeing
-  select_set(c, 0);
-  select_lane(c, 0);
-  c->stream = c->stream_main;
   esdf_destroy(c);
   mesh_destroy(c);
   icp_destroy(c);
   Tables& t = c->tab;
-  void* ptrs[] = {t.hkeys,        t.hslot,       t.htouch, t.new_list, t.touched_list,
-                  t.slot_key,     t.slot_updated, t.slot_esdf_updated, t.slot_has_esdf, t.tsdf, c->d_xyz,
-                  c->d_rgba,      c->pkeys[0],   c->pkeys[1],    c->pvals[0],   c->pvals[1], c->ckeys[0],
-                  c->ckeys[1],    c->cvals[0],   c->cvals[1],    c->order,      c->ray_p,    c->ray_c,
-                  c->cnt,         c->off,        c->set_start,  c->set_observed, c->d_state,
-                  c->ray_list,    c->head_list,  c->long_list,  c->ray_a,      c->sort_plan[0], c->sort_plan[1],
-                  c->sort_status[0], c->sort_status[1], c->scan_status, c->long_end, c->keep_bits,
-                  c->d_nblocks, c->order_inv, c->d_hold};
+  void* ptrs[] = {t.hkeys,    t.hslot,        t.htouch,       t.new_list,   t.slot_key,     t.slot_updated,
+                  t.slot_esdf_updated, t.slot_has_esdf, t.tsdf, c->order, c->order_inv, c->set_start,
+                  c->set_observed, c->d_nblocks, c->d_hold};
   for (void* p : ptrs) {
     if (p) cudaFree(p);
   }
-  if (c->h_state) cudaFreeHost(c->h_state);
   if (c->mirror_dev) cudaFree(c->mirror_dev);
   if (c->mirror_host) cudaFreeHost(c->mirror_host);
   if (c->mirror_slots) cudaFree(c->mirror_slots);
-  for (int k = 0; k < vbx_ctx::kSets; ++k) {
-    vbx_ctx::ScratchSet& S = c->set[k];
-    free_scan_blocks(&S.blocks);
-    if (k > 0) {
-      void* sp[] = {S.ray_p, S.ray_a, S.ray_c, S.ray_list, S.head_list, S.touched_list, S.cnt, S.off, S.d_state, S.d_xyz, S.d_rgba, S.pkeys0,
-                    S.ckeys[0], S.ckeys[1], S.cvals[0], S.cvals[1], S.long_list, S.long_end, S.keep_bits,
-                    S.sort_plan1, S.sort_status1};
-      for (void* p : sp) {
-        if (p) cudaFree(p);
-      }
-      if (S.h_state) cudaFreeHost(S.h_state);
-    }
-    if (S.d_args) cudaFree(S.d_args);
-    if (S.h_args) cudaFreeHost(S.h_args);
-    for (auto& per_lane : S.graph) {
-      for (vbx_ctx::ScanGraph& G : per_lane) {
-        if (G.exec) cudaGraphExecDestroy(G.exec);
-        if (G.graph) cudaGraphDestroy(G.graph);
-      }
-    }
-    if (S.stream) cudaStreamDestroy(S.stream);
-    if (S.copy_done) cudaEventDestroy(S.copy_done);
-    if (S.front_done) cudaEventDestroy(S.front_done);
-    if (S.walked) cudaEventDestroy(S.walked);
-    if (S.sorted) cudaEventDestroy(S.sorted);
-    if (S.back_done) cudaEventDestroy(S.back_done);
-    if (S.applied) cudaEventDestroy(S.applied);
-    if (S.front_start) cudaEventDestroy(S.front_start);
-  }
-  for (int l = 0; l < vbx_ctx::kLanes; ++l) {
-    vbx_ctx::FrontLane& F = c->lane[l];
-    if (l > 0) {
-      void* fp[] = {F.pkeys1, F.pvals[0], F.pvals[1], F.sort_plan0, F.sort_status0, F.scan_status};
-      for (void* p : fp) {
-        if (p) cudaFree(p);
-      }
-    }
-    free_order_scratch(&F.order_scratch, F.big_list, F.first_bits);
-    if (F.side) {
-      cudaStreamSynchronize(F.side);
-      cudaStreamDestroy(F.side);
-    }
-    if (F.ev_fork) cudaEventDestroy(F.ev_fork);
-    if (F.ev_join) cudaEventDestroy(F.ev_join);
-    if (F.done) cudaEventDestroy(F.done);
-    if (F.stream) cudaStreamDestroy(F.stream);
-  }
+  for (vbx_ctx::ScratchSet& S : c->set) free_set(S);
+  for (vbx_ctx::FrontLane& F : c->lane) free_lane(F);
   if (c->timeline_ref) cudaEventDestroy(c->timeline_ref);
   if (c->ev0) cudaEventDestroy(c->ev0);
   if (c->ev1) cudaEventDestroy(c->ev1);
@@ -645,7 +492,7 @@ void vbx_destroy(vbx_ctx* c) {
   for (int i = 0; i < 20; ++i) {
     if (c->sev[i]) cudaEventDestroy(c->sev[i]);
   }
-  if (c->stream_main) cudaStreamDestroy(c->stream_main);
+  if (c->stream) cudaStreamDestroy(c->stream);
   if (c->stream_e) cudaStreamDestroy(c->stream_e);
   if (c->stream_s) cudaStreamDestroy(c->stream_s);
   for (cudaEvent_t e : c->cap_ev) {
@@ -667,7 +514,7 @@ int vbx_tsdf_integrate_device(vbx_ctx* c, int kind, const float q[4], const floa
   if (!c || !q || !t || (n && (!d_xyz || !d_rgba))) return fail(c, VBX_E_INVALID, "null argument");
   VBX_CUDA(c, cudaSetDevice(c->device));
   VBX_DRAIN(c);
-  return integrate_device(c, kind, q, t, d_xyz, d_rgba, n, freespace);
+  return integrate_device(c, sync_route(c), kind, q, t, d_xyz, d_rgba, n, freespace);
 }
 
 int vbx_tsdf_integrate(vbx_ctx* c, int kind, const float q[4], const float t[3], const float* xyz,
@@ -676,18 +523,19 @@ int vbx_tsdf_integrate(vbx_ctx* c, int kind, const float q[4], const float t[3],
   if (n > c->max_points) return fail(c, VBX_E_CAPACITY, "cloud larger than max_points_per_scan");
   VBX_CUDA(c, cudaSetDevice(c->device));
   VBX_DRAIN(c);
+  const vbx_ctx::ScratchSet& S = c->set[0];
   if (n) {
-    VBX_CUDA(c, cudaMemcpyAsync(c->d_xyz, xyz, n * 3 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    VBX_CUDA(c, cudaMemcpyAsync(c->d_rgba, rgba, n * 4, cudaMemcpyHostToDevice, c->stream));
+    VBX_CUDA(c, cudaMemcpyAsync(S.d_xyz, xyz, n * 3 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    VBX_CUDA(c, cudaMemcpyAsync(S.d_rgba, rgba, n * 4, cudaMemcpyHostToDevice, c->stream));
   }
-  return integrate_device(c, kind, q, t, c->d_xyz, c->d_rgba, n, freespace);
+  return integrate_device(c, sync_route(c), kind, q, t, S.d_xyz, S.d_rgba, n, freespace);
 }
 
 int vbx_tsdf_integrate_async(vbx_ctx* c, int kind, const float q[4], const float t[3], const float* xyz,
                              const uint8_t* rgba, uint64_t n, int freespace, int inputs_on_device) {
   if (!c || !q || !t || (n && (!xyz || !rgba))) return fail(c, VBX_E_INVALID, "null argument");
   if (cudaSetDevice(c->device) != cudaSuccess) return fail(c, VBX_E_CUDA, "cudaSetDevice");
-  return integrate_async(c, kind, q, t, xyz, rgba, n, freespace, inputs_on_device);
+  return integrate_async(c, sync_route(c), kind, q, t, xyz, rgba, n, freespace, inputs_on_device);
 }
 
 int vbx_block_owner(const vbx_ctx* c, const int32_t block_index[3], int32_t* owner) {
@@ -808,7 +656,7 @@ int vbx_host_copy_ms(vbx_ctx* c, const void* src, size_t bytes, float* ms) {
   VBX_CUDA(c, cudaSetDevice(c->device));
   VBX_DRAIN(c);
   VBX_CUDA(c, cudaEventRecord(c->tev0, c->stream));
-  VBX_CUDA(c, cudaMemcpyAsync(c->d_xyz, src, bytes, cudaMemcpyHostToDevice, c->stream));
+  VBX_CUDA(c, cudaMemcpyAsync(c->set[0].d_xyz, src, bytes, cudaMemcpyHostToDevice, c->stream));
   VBX_CUDA(c, cudaEventRecord(c->tev1, c->stream));
   VBX_CUDA(c, cudaEventSynchronize(c->tev1));
   VBX_CUDA(c, cudaEventElapsedTime(ms, c->tev0, c->tev1));
@@ -852,7 +700,7 @@ int vbx_sync(vbx_ctx* c) {
   if (!c) return VBX_E_INVALID;
   VBX_CUDA(c, cudaSetDevice(c->device));
   VBX_DRAIN(c);
-  VBX_CUDA(c, cudaStreamSynchronize(c->stream_main));  // (the drain above already waited for every queued scan)
+  VBX_CUDA(c, cudaStreamSynchronize(c->stream));  // (the drain above already waited for every queued scan)
   return VBX_OK;
 }
 

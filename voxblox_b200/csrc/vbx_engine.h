@@ -177,8 +177,7 @@ __host__ __device__ inline uint32_t hash64(uint64_t k) {
 
 struct vbx_ctx {
   int device = 0;
-  cudaStream_t stream = nullptr;      // the stream the next launch goes to (main, or a pipeline stage's stream while one is enqueued)
-  cudaStream_t stream_main = nullptr; // back halves, ESDF, block management, synchronous calls
+  cudaStream_t stream = nullptr;      // main stream: synchronous calls, ESDF, block management, pipelined applies
   cudaStream_t stream_c = nullptr;    // host-to-device cloud copies of asynchronously submitted scans
   cudaStream_t stream_c2 = nullptr;   // ... alternating with this one
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -189,8 +188,7 @@ struct vbx_ctx {
   uint32_t vox_per_block = 4096;
   uint32_t hcap = 0;
   unsigned int grid_sms = 132;  // persistent-kernel grids are multiples of this (the device's SM count, queried at create; VBX_GRID_SMS overrides: tuning aid)
-  vbx::Tables tab;
-  vbx::ScanBlocks blocks{};  // the current hand-off set's private block table
+  vbx::Tables tab;  // the map (touched_list is null: each hand-off set owns its own)
   // scratch
   uint32_t max_points = 0;
   uint64_t max_updates = 0;
@@ -198,44 +196,16 @@ struct vbx_ctx {
   cudaEvent_t timeline_ref = nullptr;
   uint32_t bundle_hint = 0;         // bundles (the larger of the two maps) of the most recent Merged scan whose counters reached the host
   uint64_t record_hint = 1u << 20;  // update records of the most recent scan whose count reached the host: sizes the record sort's grid
-  float* d_xyz = nullptr;
-  uint8_t* d_rgba = nullptr;
-  uint64_t* pkeys[2] = {nullptr, nullptr};
-  uint32_t* pvals[2] = {nullptr, nullptr};
-  uint32_t* order = nullptr;
-  uint32_t* order_inv = nullptr;           // [max_points] inverse of `order` ("sorted" integration order)
-  uint32_t* ray_list = nullptr;            // [max_points] Merged: ray slot (rank in the reference's bundle order) -> head
-  uint32_t* head_list = nullptr;           // [max_points] bundle heads, unordered (hand-off set private)
-  uint32_t* big_list = nullptr;            // [max_points / 256 + 1] ids of the big bundles (front-lane private)
-  cudaStream_t side_stream = nullptr;      // k_bundle_order runs here, beside k_merge (front-lane private)
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-  uint32_t* first_bits = nullptr;          // [2][max_points / 32 + 1] first-occurrence bitmaps (front-lane private)
-  vbx::OrderScratch order_scratch{};         // k_bundle_order's global tables (front-lane private)
+  uint32_t* order = nullptr;               // [max_points] "sorted" integration order
+  uint32_t* order_inv = nullptr;           // [max_points] inverse of `order`
   vbx::RehashSchedule rehash{};            // libstdc++'s unordered_map growth schedule (vbx_create)
   size_t order_smem_bytes = 0;             // dynamic shared memory of k_bundle_order
-  unsigned long long* long_list = nullptr; // [max_updates / 32 + 1] first record of each long voxel run (hand-off set private)
-  unsigned long long* long_end = nullptr;  // [max_updates / 32 + 1] one past its last record
-  uint32_t* keep_bits = nullptr;           // [max_updates / 32 + 1] per sorted record: the update keeps (+T, max_weight)
-  float4* ray_p = nullptr;    // point_G.xyz, flags (bit 0: clearing ray)
-  float4* ray_a = nullptr;    // point_G - origin, |point_G - origin|
-  uint2* ray_c = nullptr;     // colour, weight bits
-  uint32_t* cnt = nullptr;    // [max_points + 1]
-  uint32_t* off = nullptr;    // [max_points + 1]
-  uint32_t* ckeys[2] = {nullptr, nullptr};
-  uint32_t* cvals[2] = {nullptr, nullptr};
-  // the engine's own radix sort / scan (vbx_sort.cuh): [0] point keys, [1] update records
-  vbx::SortPlan* sort_plan[2] = {nullptr, nullptr};
-  uint32_t* sort_status[2] = {nullptr, nullptr};
+  // tiles of the engine's own radix sorts (vbx_sort.cuh): [0] point keys, [1] update records
   uint32_t sort_tiles_cap[2] = {0, 0};
-  uint32_t* scan_status = nullptr;
   unsigned long long* set_start = nullptr;  // Fast integrator approximate sets
   unsigned long long* set_observed = nullptr;
   uint32_t set_epoch = 1;
   int64_t fast_reset_counter = 0;
-  vbx::ScanState* d_state = nullptr;
-  vbx::ScanState* h_state = nullptr;  // pinned
-  vbx::ScanArgs* d_args = nullptr;    // the current hand-off set's argument block ...
-  vbx::ScanArgs* h_args = nullptr;    // ... and its page-locked host copy
   uint32_t epoch = 0;                 // call id for touch marks
   uint32_t n_blocks = 0;              // pool slots in use (host copy, exact after a drain)
   uint32_t* d_nblocks = nullptr;      // [2] device copy, ping-pong: k_assign reads [nb_cur], writes [nb_cur ^ 1]
@@ -244,8 +214,9 @@ struct vbx_ctx {
   // (keys, bundle sort, bundle fold, offsets, Merged's ray trace; does not touch the map) on one of kLanes
   // front lanes, block creation, record sort, apply -- so up to kSets scans are in flight, each owning one set
   // of hand-off buffers.  Map-touching stages run in submission order.  Each scan is one launch of a CUDA
-  // graph per (hand-off set, front lane, kind), captured before its first use.  Set 0 / lane 0 are the
-  // buffers the synchronous calls use; the others are allocated on the first asynchronous submission.
+  // graph per (hand-off set, front lane, kind), captured before its first use.  The sets and lanes are the
+  // only owners of per-scan scratch: set 0 / lane 0 (allocated by vbx_create) are the buffers the synchronous
+  // calls use, the others are allocated on the first asynchronous submission (alloc_set / alloc_lane).
   static constexpr int kSets = 16, kLanes = 8;  // upper bounds
   int sets_in_use = 10, lanes_in_use = 6;  // (tuning aids: VBX_ASYNC_SETS, VBX_ASYNC_LANES)
   enum { kGraphSimple, kGraphMerged, kGraphVariants };
@@ -262,28 +233,30 @@ struct vbx_ctx {
     size_t order_smem = 0;
   };
   struct ScratchSet {
-    float4* ray_p = nullptr;
-    float4* ray_a = nullptr;
-    uint2* ray_c = nullptr;
-    uint32_t* ray_list = nullptr;
+    float4* ray_p = nullptr;         // [max_points] point_G.xyz, flags (bit 0: clearing ray)
+    float4* ray_a = nullptr;         // [max_points] point_G - origin, |point_G - origin|
+    uint2* ray_c = nullptr;          // [max_points] colour, weight bits
+    uint32_t* ray_list = nullptr;    // [max_points] Merged: ray slot (rank in the reference's bundle order) -> head
     uint32_t* head_list = nullptr;   // bundle id -> sorted position of its head (read again by the ray walk)
     uint32_t* touched_list = nullptr;  // touched id -> hash position (written by k_assign / the walk, read by the apply)
     vbx::ScanBlocks blocks{};          // Merged: local block ids of the trace (written by the front half, read by k_assign)
-    uint32_t* cnt = nullptr;
-    uint32_t* off = nullptr;
+    uint32_t* cnt = nullptr;         // [max_points + 1]
+    uint32_t* off = nullptr;         // [max_points + 1]
     vbx::ScanState* d_state = nullptr;
-    vbx::ScanState* h_state = nullptr;
+    vbx::ScanState* h_state = nullptr;  // page-locked
     vbx::ScanArgs* d_args = nullptr;
     vbx::ScanArgs* h_args = nullptr;  // page-locked: the graph's first node uploads it
-    float* d_xyz = nullptr;
+    float* d_xyz = nullptr;          // a host cloud's device copy
     uint8_t* d_rgba = nullptr;
     uint64_t* pkeys0 = nullptr;  // sorted bundle keys (read again by the ray walk)
     uint32_t* ckeys[2] = {nullptr, nullptr};  // update records (written by the walk, read by apply)
     uint32_t* cvals[2] = {nullptr, nullptr};
-    unsigned long long* long_list = nullptr;  // long voxel runs and keep bits of the sorted records (k_apply_prep -> k_apply)
+    // [max_updates / 32 + 1] each: the long voxel runs' first record and end, and per sorted record a bit
+    // "the update keeps (+T, max_weight)" (k_apply_prep -> k_apply)
+    unsigned long long* long_list = nullptr;
     unsigned long long* long_end = nullptr;
     uint32_t* keep_bits = nullptr;
-    vbx::SortPlan* sort_plan1 = nullptr;
+    vbx::SortPlan* sort_plan1 = nullptr;  // the record sort's plan and status words
     uint32_t* sort_status1 = nullptr;
     cudaEvent_t copy_done = nullptr, walked = nullptr, sorted = nullptr, applied = nullptr, back_done = nullptr;
     cudaEvent_t front_start = nullptr, front_done = nullptr;  // only with VBX_ASYNC_TIMELINE (vbx_debug_async_timeline)
@@ -304,15 +277,15 @@ struct vbx_ctx {
   } set[kSets];
   struct FrontLane {  // scratch private to one front-half stream
     cudaStream_t stream = nullptr;
-    uint64_t* pkeys1 = nullptr;
+    uint64_t* pkeys1 = nullptr;  // the point sort's second key buffer
     uint32_t* pvals[2] = {nullptr, nullptr};
-    vbx::SortPlan* sort_plan0 = nullptr;
+    vbx::SortPlan* sort_plan0 = nullptr;  // the point sort's plan and status words
     uint32_t* sort_status0 = nullptr;
-    uint32_t* scan_status = nullptr;
-    uint32_t* big_list = nullptr;
-    uint32_t* first_bits = nullptr;
-    vbx::OrderScratch order_scratch{};
-    cudaStream_t side = nullptr;
+    uint32_t* scan_status = nullptr;  // the offset scan's tile status words
+    uint32_t* big_list = nullptr;     // [max_points / 256 + 1] ids of the big bundles
+    uint32_t* first_bits = nullptr;   // [2][max_points / 32 + 1] first-occurrence bitmaps
+    vbx::OrderScratch order_scratch{};  // k_bundle_order's global tables
+    cudaStream_t side = nullptr;      // k_bundle_order runs here, beside k_merge
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     cudaEvent_t done = nullptr;  // the lane's last front half
   } lane[kLanes];
@@ -321,14 +294,6 @@ struct vbx_ctx {
   // the streams a scan's graph is captured from (besides the front lane's and the main stream)
   cudaStream_t stream_e = nullptr;  // block creation: k_back_begin, k_assign (Simple: and its ray walk)
   cudaStream_t stream_s = nullptr;  // record sort + apply preparation
-  // non-null while a scan's graph is captured: the back half's streams and hand-off events (integrate_async)
-  struct Capture {
-    cudaStream_t sort, apply;
-    cudaEvent_t walked, sorted, applied;   // this scan's stage ends: later scans' graphs wait for them
-    cudaEvent_t prev_sorted, prev_applied; // the record sort two scans back, the previous scan's apply
-    cudaEvent_t edge[2];                   // capture-internal: walk -> sort, sort -> apply
-  };
-  const Capture* cap = nullptr;
   cudaEvent_t cap_ev[8] = {};  // capture-internal edges (fork, front -> walk, walk -> sort, sort -> apply, joins)
   uint64_t async_seq = 0;
   uint32_t* d_hold = nullptr;           // device flag: a queued scan must be redone, later scans skip their back half
@@ -417,18 +382,26 @@ int mesh_download(vbx_ctx* c, int32_t* idx3, uint64_t* first_vertex, float* vert
 int esdf_add_robot_position(vbx_ctx* c, const float p[3]);
 int esdf_clear_state(vbx_ctx* c);
 int ensure_async(vbx_ctx* c);          // allocate the extra hand-off sets / front lanes
-void select_set(vbx_ctx* c, int k);     // point the context's scratch fields at hand-off set k / front lane l
-void select_lane(vbx_ctx* c, int l);
 int drain_async(vbx_ctx* c);           // wait for every asynchronously submitted scan, collect its results
 int set_n_blocks(vbx_ctx* c, uint32_t n);
-int alloc_order_scratch(vbx_ctx* c, vbx::OrderScratch* g, uint32_t** big_list, uint32_t** first_bits);
-void free_order_scratch(vbx::OrderScratch* g, uint32_t* big_list, uint32_t* first_bits);
-int alloc_scan_blocks(vbx_ctx* c, vbx::ScanBlocks* b);  // a hand-off set's private block table, zeroed
-void free_scan_blocks(vbx::ScanBlocks* b);
 int init_bundle_order(vbx_ctx* c);     // rehash schedule + shared-memory opt-in of k_bundle_order
 int rebuild_hash(vbx_ctx* c);          // block hash rebuilt from slot_key (after removals / a pool overflow)
 void harvest_async(vbx_ctx* c, vbx_ctx::ScratchSet& S);  // collect a finished asynchronous scan's results
 int alloc_scan_args(vbx_ctx* c, vbx_ctx::ScratchSet& S);  // the set's argument block, device + page-locked host
+
+// Where a scan's work is enqueued (vbx_tsdf.cu): its hand-off set and front lane, the stream of the stage
+// being enqueued, the unit of the persistent kernels' grids and whether stage marks are recorded.
+struct ScanRoute {
+  vbx_ctx::ScratchSet& S;
+  vbx_ctx::FrontLane& F;
+  cudaStream_t s;
+  unsigned int sms;  // an SM count: the whole GPU, or a share of it in the pipelined graphs
+  bool marks;        // vbx_set_stage_profiling
+};
+// The synchronous calls: hand-off set 0 and front lane 0 on the main stream, grids for the whole GPU.
+inline ScanRoute sync_route(vbx_ctx* c) { return {c->set[0], c->lane[0], c->stream, c->grid_sms, c->profiling}; }
+int integrate_device(vbx_ctx* c, const ScanRoute& x, int kind, const float q[4], const float t[3], const float* d_xyz,
+                     const uint8_t* d_rgba, uint64_t n, int freespace);
 }  // namespace vbx
 
 #define VBX_CUDA(c, expr)                                          \

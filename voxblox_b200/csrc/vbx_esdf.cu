@@ -849,30 +849,31 @@ int esdf_add_robot_position(vbx_ctx* c, const float p[3]) {
   }
   // the per-axis lists ride in the seed-value scratch (floats; frontier_cap >> 1300 entries)
   float* d_xs[2] = {c->esdf_seed_val, c->esdf_seed_val + xs[0].size()};
+  ScanState* d_state = c->set[0].d_state;  // hand-off set 0's status block
   VBX_CUDA(c, cudaEventRecord(c->ev0, s));
-  VBX_CUDA(c, cudaMemsetAsync(c->d_state, 0, sizeof(ScanState), s));
-  k_esdf_set_pending<<<1, 1, 0, s>>>(c->d_state, c->esdf_pending_raise, c->esdf_pending_open);
+  VBX_CUDA(c, cudaMemsetAsync(d_state, 0, sizeof(ScanState), s));
+  k_esdf_set_pending<<<1, 1, 0, s>>>(d_state, c->esdf_pending_raise, c->esdf_pending_open);
   for (int k = 0; k < 2; ++k) {
     if (S[k].n == 0) continue;
     VBX_CUDA(c, cudaMemcpyAsync(d_xs[k], xs[k].data(), xs[k].size() * sizeof(float), cudaMemcpyHostToDevice, s));
     const uint64_t n3 = (uint64_t)S[k].n * S[k].n * S[k].n;
-    k_esdf_sphere_blocks<<<grid_for(n3, 256), 256, 0, s>>>(S[k], c->tab, d_xs[k], c->d_state);
+    k_esdf_sphere_blocks<<<grid_for(n3, 256), 256, 0, s>>>(S[k], c->tab, d_xs[k], d_state);
     launches += 1;
   }
-  k_esdf_sphere_assign<<<grid_for(c->tab.max_blocks, 256), 256, 0, s>>>(c->tab, c->n_blocks, c->d_state);
+  k_esdf_sphere_assign<<<grid_for(c->tab.max_blocks, 256), 256, 0, s>>>(c->tab, c->n_blocks, d_state);
   launches += 2;
   for (int k = 0; k < 2; ++k) {
     if (S[k].n == 0) continue;
     const uint64_t n3 = (uint64_t)S[k].n * S[k].n * S[k].n;
-    k_esdf_sphere_apply<<<grid_for(n3, 256), 256, 0, s>>>(S[k], c->tab, d_xs[k], c->raise_q[0], c->frontier[0], c->d_state);
+    k_esdf_sphere_apply<<<grid_for(n3, 256), 256, 0, s>>>(S[k], c->tab, d_xs[k], c->raise_q[0], c->frontier[0], d_state);
     launches += 1;
   }
   VBX_CUDA(c, cudaEventRecord(c->ev1, s));
-  VBX_CUDA(c, cudaMemcpyAsync(c->h_state, c->d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(c->set[0].h_state, d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));  // (also keeps xs[] alive until the copies are done)
   VBX_CUDA(c, cudaGetLastError());
   VBX_CUDA(c, cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
-  const ScanState& h = *c->h_state;
+  const ScanState& h = *c->set[0].h_state;
   if (h.error & (kErrPoolFull | kErrHashFull)) return fail(c, VBX_E_CAPACITY, "block pool / hash full in addNewRobotPosition");
   if (h.error & kErrCoordRange) return fail(c, VBX_E_INVALID, "robot position sphere outside the +-2^20 block range");
   if (h.error & kErrUpdatesFull) return fail(c, VBX_E_CAPACITY, "ESDF wavefront queue capacity exceeded");
@@ -944,9 +945,11 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
     VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_fe),
                            (size_t)c->tab.max_blocks * c->vox_per_block * sizeof(unsigned long long)));
   }
+  ScanState* d_state = c->set[0].d_state;  // hand-off set 0's status block
+  const ScanState& h = *c->set[0].h_state;
   VBX_CUDA(c, cudaEventRecord(c->ev0, s));
   if (c->profiling) cudaEventRecord(c->sev[0], s);
-  VBX_CUDA(c, cudaMemsetAsync(c->d_state, 0, sizeof(ScanState), s));
+  VBX_CUDA(c, cudaMemsetAsync(d_state, 0, sizeof(ScanState), s));
   if (c->n_blocks == 0) {
     VBX_CUDA(c, cudaStreamSynchronize(s));
     return VBX_OK;
@@ -960,7 +963,7 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
   // head of raise_q[0] / frontier[0]; this call's own entries are appended behind them)
   const bool pending = c->esdf_pending_raise || c->esdf_pending_open;
   if (pending) {
-    k_esdf_set_pending<<<1, 1, 0, s>>>(c->d_state, c->esdf_pending_raise, c->esdf_pending_open);
+    k_esdf_set_pending<<<1, 1, 0, s>>>(d_state, c->esdf_pending_raise, c->esdf_pending_open);
     launches += 1;
   }
   c->esdf_pending_raise = c->esdf_pending_open = 0;
@@ -976,7 +979,7 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
     nb = n_listed;
     if (nb > 0) {
       VBX_CUDA(c, cudaMemcpyAsync(c->esdf_block_list, listed_slots, (size_t)nb * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-      VBX_CUDA(c, cudaMemcpyAsync(&c->d_state->esdf_counts[0], &nb, sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+      VBX_CUDA(c, cudaMemcpyAsync(&d_state->esdf_counts[0], &nb, sizeof(uint32_t), cudaMemcpyHostToDevice, s));
       k_esdf_mark_listed<<<grid_for(nb, 256), 256, 0, s>>>(c->tab, c->esdf_block_list, nb);
       VBX_CUDA(c, cudaStreamSynchronize(s));  // the two host sources above are stack / vector memory
     }
@@ -984,7 +987,7 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
     // the list and its length (esdf_counts[0]) stay on the device: no host round trip in the middle of
     // the call; the launches below are sized for the upper bound (every slot) and the kernels stop at
     // the real count
-    k_esdf_block_list<<<grid_for(c->n_blocks, 256), 256, 0, s>>>(c->tab, c->n_blocks, batch, c->esdf_block_list, c->d_state);
+    k_esdf_block_list<<<grid_for(c->n_blocks, 256), 256, 0, s>>>(c->tab, c->n_blocks, batch, c->esdf_block_list, d_state);
     nb = c->n_blocks;
   }
   launches += 1;
@@ -993,13 +996,13 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
       // one thread block per voxel block, both slabs staged by the TMA
       const size_t slab_bytes = (size_t)c->vox_per_block * (sizeof(TsdfVoxel) + sizeof(EsdfVoxel));
       k_esdf_propagate<<<nb, (unsigned int)std::max<uint32_t>(32u, std::min<uint32_t>(1024u, c->vox_per_block)), slab_bytes, s>>>(
-          E, c->tab, c->esdf_block_list, nb, c->frontier[0], c->raise_q[0], c->esdf_seed_list, c->d_state);
+          E, c->tab, c->esdf_block_list, nb, c->frontier[0], c->raise_q[0], c->esdf_seed_list, d_state);
       launches += 1;
     }
     if (nb > 0 && incremental) {
       const unsigned int g = c->grid_sms * 8;
-      k_esdf_seed<<<g, 256, 0, s>>>(E, c->tab, c->esdf_seed_list, c->frontier[0], c->esdf_seed_val, c->d_state);
-      k_esdf_seed_commit<<<g, 256, 0, s>>>(E, c->tab, c->esdf_seed_list, c->esdf_seed_val, c->d_state);
+      k_esdf_seed<<<g, 256, 0, s>>>(E, c->tab, c->esdf_seed_list, c->frontier[0], c->esdf_seed_val, d_state);
+      k_esdf_seed_commit<<<g, 256, 0, s>>>(E, c->tab, c->esdf_seed_list, c->esdf_seed_val, d_state);
       launches += 2;
     }
     if (c->profiling) cudaEventRecord(c->sev[1], s);
@@ -1009,30 +1012,30 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
       c->esdf_grid_raise = c->esdf_grid_lower = c->esdf_sms * per_sm;
     }
     {
-      void* args[] = {&E, &c->tab, &c->raise_q[0], &c->raise_q[1], &c->frontier[0], &c->d_state};
+      void* args[] = {&E, &c->tab, &c->raise_q[0], &c->raise_q[1], &c->frontier[0], &d_state};
       VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_esdf_raise, dim3(c->esdf_grid_raise), dim3(256), args, 0, s));
     }
     if (c->profiling) cudaEventRecord(c->sev[2], s);
     long long* fe = nullptr;
     if (E.full_euclidean) {
       fe = reinterpret_cast<long long*>(c->esdf_fe);
-      k_esdf_fe_pack<<<c->grid_sms * 8, 256, 0, s>>>(c->tab, (uint64_t)c->n_blocks * c->vox_per_block, fe, c->d_state);
+      k_esdf_fe_pack<<<c->grid_sms * 8, 256, 0, s>>>(c->tab, (uint64_t)c->n_blocks * c->vox_per_block, fe, d_state);
       launches += 1;
     }
     {
-      void* args[] = {&E, &c->tab, &c->frontier[0], &c->frontier[1], &c->esdf_touched, &fe, &c->d_state};
+      void* args[] = {&E, &c->tab, &c->frontier[0], &c->frontier[1], &c->esdf_touched, &fe, &d_state};
       VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_esdf_lower, dim3(c->esdf_grid_lower), dim3(256), args, 0, s));
     }
-    k_esdf_parents<<<c->grid_sms * 8, 256, 0, s>>>(E, c->tab, c->esdf_touched, fe, c->d_state);
+    k_esdf_parents<<<c->grid_sms * 8, 256, 0, s>>>(E, c->tab, c->esdf_touched, fe, d_state);
     if (c->profiling) cudaEventRecord(c->sev[3], s);
     launches += 3;
     if (nb > 0 && !batch && clear_updated_flag) {
-      k_esdf_clear_tsdf_flag<<<grid_for(nb, 256), 256, 0, s>>>(c->tab, c->esdf_block_list, c->d_state);
+      k_esdf_clear_tsdf_flag<<<grid_for(nb, 256), 256, 0, s>>>(c->tab, c->esdf_block_list, d_state);
       launches += 1;
     }
   }
   VBX_CUDA(c, cudaEventRecord(c->ev1, s));
-  VBX_CUDA(c, cudaMemcpyAsync(c->h_state, c->d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(c->set[0].h_state, d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));
   VBX_CUDA(c, cudaGetLastError());
   VBX_CUDA(c, cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
@@ -1045,11 +1048,11 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
       }
     }
   }
-  if (c->h_state->error & kErrUpdatesFull) return fail(c, VBX_E_CAPACITY, "ESDF wavefront queue capacity exceeded");
-  if (c->h_state->error & kErrParentRange) {
+  if (h.error & kErrUpdatesFull) return fail(c, VBX_E_CAPACITY, "ESDF wavefront queue capacity exceeded");
+  if (h.error & kErrParentRange) {
     return fail(c, VBX_E_CAPACITY, "full-Euclidean ESDF: a parent vector component left [-512, 511] voxels");
   }
-  for (int i = 0; i < 7; ++i) c->esdf_counters[i] = c->h_state->esdf_counts[i];
+  for (int i = 0; i < 7; ++i) c->esdf_counters[i] = h.esdf_counts[i];
   c->esdf_counters[7] = launches;
   c->launches += launches;
   return VBX_OK;

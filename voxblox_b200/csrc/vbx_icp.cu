@@ -522,7 +522,7 @@ int icp_run(vbx_ctx* c, const vbx_icp_config* cfg, const float* points, int on_d
     VBX_CUDA(c, cudaHostAlloc(reinterpret_cast<void**>(&c->icp_out_host), 16 * sizeof(float), cudaHostAllocDefault));
     c->icp_cap = cap;
   }
-  cudaStream_t s = c->stream_main;
+  cudaStream_t s = c->stream;
   const float* d_points = points;
   if (!on_device && n) {
     VBX_CUDA(c, cudaMemcpyAsync(c->icp_points_dev, points, n * 3 * sizeof(float), cudaMemcpyHostToDevice, s));

@@ -2138,12 +2138,12 @@ int init_bundle_order(vbx_ctx* c) {
 
 static inline unsigned int grid_for(uint64_t n, int block) { return (unsigned int)((n + block - 1) / block); }
 
-static int check_state_errors(vbx_ctx* c, uint32_t err) {
-  err &= kFatalErrors;
+static int check_state_errors(vbx_ctx* c, const ScanState& h) {
+  const uint32_t err = h.error & kFatalErrors;
   if (!err) return VBX_OK;
   if (err & kErrPoolFull) {
     // the surplus hash entries of this call have no pool slot: drop them, or later calls would find them
-    if (c->h_state->n_blocks) c->n_blocks = c->h_state->n_blocks;
+    if (h.n_blocks) c->n_blocks = h.n_blocks;
     rebuild_hash(c);
   }
   std::string m = "device reported:";
@@ -2158,13 +2158,14 @@ namespace {
 struct Marks {
   vbx_ctx* c;
   cudaStream_t s;
+  bool on;  // (off while a graph is captured: stage events would serialise the streams)
   int n = 0;
   int stage[20];
   void begin() {
-    if (c->profiling) cudaEventRecord(c->sev[0], s);
+    if (on) cudaEventRecord(c->sev[0], s);
   }
   void mark(int stage_just_finished) {
-    if (c->profiling && n < 19) {
+    if (on && n < 19) {
       cudaEventRecord(c->sev[n + 1], s);
       stage[n++] = stage_just_finished;
     }
@@ -2179,27 +2180,43 @@ struct Marks {
     }
   }
 };
+
+// The back half's streams and hand-off events while a pipelined scan's graph is captured (capture_scan)
+struct Capture {
+  cudaStream_t sort, apply;
+  cudaEvent_t walked, sorted, applied;   // this scan's stage ends: later scans' graphs wait for them
+  cudaEvent_t prev_sorted, prev_applied; // the record sort two scans back, the previous scan's apply
+  cudaEvent_t edge[2];                   // capture-internal: walk -> sort, sort -> apply
+};
 }  // namespace
 
-static unsigned int sort_grid(const vbx_ctx* c, int which, uint64_t n_hint) {
+// The map's tables as a scan's kernels see them: with the hand-off set's touched-id list
+static Tables scan_tables(const vbx_ctx* c, const vbx_ctx::ScratchSet& S) {
+  Tables t = c->tab;
+  t.touched_list = S.touched_list;
+  return t;
+}
+
+static unsigned int sort_grid(const vbx_ctx* c, int which, uint64_t n_hint, unsigned int sms) {
   const uint64_t tiles_hint = std::max<uint64_t>(1, (n_hint + kSortTile - 1) / kSortTile);
-  return (unsigned int)std::min<uint64_t>(std::min<uint64_t>(c->sort_tiles_cap[which], tiles_hint), (uint64_t)c->grid_sms * 2);
+  return (unsigned int)std::min<uint64_t>(std::min<uint64_t>(c->sort_tiles_cap[which], tiles_hint), (uint64_t)sms * 2);
 }
 
 // The engine's own stable radix sort (vbx_sort.cuh): one launch.  n lives on the device (d_n) or is n_fixed;
 // n_hint sizes the grid (tiles are handed out by ticket, so any grid sorts any n).  result_in_a: the sorted
 // pairs end in buffer A whatever the number of passes (otherwise SortPlan::final_buf says where they are).
+// which: 0 the point sort (the front lane's plan), 1 the record sort (the hand-off set's).
 template <typename KeyT>
-static int own_sort(vbx_ctx* c, int which, KeyT* keys_a, uint32_t* vals_a, KeyT* keys_b, uint32_t* vals_b,
-                    const unsigned long long* d_n, uint32_t n_fixed, uint64_t n_hint, int key_bits, bool result_in_a,
-                    uint64_t* launches, const uint32_t* d_key_bits = nullptr, bool plan_cleared = false) {
-  cudaStream_t s = c->stream;
+static int own_sort(vbx_ctx* c, const ScanRoute& x, int which, KeyT* keys_a, uint32_t* vals_a, KeyT* keys_b,
+                    uint32_t* vals_b, const unsigned long long* d_n, uint32_t n_fixed, uint64_t n_hint, int key_bits,
+                    bool result_in_a, uint64_t* launches, const uint32_t* d_key_bits = nullptr, bool plan_cleared = false) {
+  cudaStream_t s = x.s;
   const int passes = std::min(kMaxPasses, (key_bits + 7) / 8);
-  SortPlan* plan = c->sort_plan[which];
-  uint32_t* status = c->sort_status[which];
+  SortPlan* plan = which ? x.S.sort_plan1 : x.F.sort_plan0;
+  uint32_t* status = which ? x.S.sort_status1 : x.F.sort_status0;
   const uint32_t tiles_cap = c->sort_tiles_cap[which];
   if (!plan_cleared) VBX_CUDA(c, cudaMemsetAsync(plan, 0, sizeof(SortPlan), s));  // (else: an earlier kernel of the stream did)
-  const unsigned int grid = sort_grid(c, which, n_hint);
+  const unsigned int grid = sort_grid(c, which, n_hint, x.sms);
   k_sort<KeyT><<<grid, kSortThreads, 0, s>>>(keys_a, vals_a, keys_b, vals_b, d_n, n_fixed, passes, d_key_bits, plan, status,
                                               tiles_cap, result_in_a ? 1 : 0);
   *launches += 1;
@@ -2234,10 +2251,13 @@ static OrderLaunch order_launch(const vbx_ctx* c, uint32_t n) {
 }
 
 template <typename KeyT>
-static int launch_bundle_order(vbx_ctx* c, cudaStream_t so, uint32_t n, const KeyT* keys, const uint32_t* vals) {
-  k_order_prefix<<<1, kOrderThreads, 0, so>>>(c->d_args, c->first_bits, c->order_scratch, c->d_state);
-  k_order_heads<KeyT><<<std::min<unsigned int>(grid_for(c->max_points, 256), c->grid_sms * 2), 256, 0, so>>>(
-      c->d_args, keys, vals, c->order_inv, c->head_list, c->first_bits, c->order_scratch, c->d_state);
+static int launch_bundle_order(vbx_ctx* c, const ScanRoute& x, cudaStream_t so, uint32_t n, const KeyT* keys,
+                               const uint32_t* vals) {
+  const vbx_ctx::ScratchSet& S = x.S;
+  const vbx_ctx::FrontLane& F = x.F;
+  k_order_prefix<<<1, kOrderThreads, 0, so>>>(S.d_args, F.first_bits, F.order_scratch, S.d_state);
+  k_order_heads<KeyT><<<std::min<unsigned int>(grid_for(c->max_points, 256), x.sms * 2), 256, 0, so>>>(
+      S.d_args, keys, vals, c->order_inv, S.head_list, F.first_bits, F.order_scratch, S.d_state);
   // Always a cooperative launch (the one-block form is a cooperative grid of one block), so that a scan
   // graph's node switches between the two forms by its grid and shared memory alone (update_scan_graph).
   const OrderLaunch o = order_launch(c, n);
@@ -2252,8 +2272,8 @@ static int launch_bundle_order(vbx_ctx* c, cudaStream_t so, uint32_t n, const Ke
   coop.val.cooperative = 1;
   lc.attrs = &coop;
   lc.numAttrs = 1;
-  VBX_CUDA(c, cudaLaunchKernelEx(&lc, k_bundle_order, c->rehash, c->order_scratch, smem_words, c->ray_list,
-                                 c->order_scratch.cta_tot, c->d_state));
+  VBX_CUDA(c, cudaLaunchKernelEx(&lc, k_bundle_order, c->rehash, F.order_scratch, smem_words, S.ray_list,
+                                 F.order_scratch.cta_tot, S.d_state));
   return VBX_OK;
 }
 
@@ -2262,22 +2282,26 @@ static int launch_bundle_order(vbx_ctx* c, cudaStream_t so, uint32_t n, const Ke
 static bool traced_in_front(const ScanParams& P) { return P.kind == VBX_MERGED && P.single_walk; }
 
 template <typename KeyT>
-static void launch_trace(vbx_ctx* c, const KeyT* keys, cudaStream_t s) {
+static void launch_trace(const ScanRoute& x, const KeyT* keys) {
   // a few thousand bundles of 100-300 steps: one warp per ray
-  k_rays_emit_warp<KeyT><<<c->grid_sms * 8, 128, 0, s>>>(c->d_args, c->blocks, keys, c->ray_list, c->head_list, c->ray_p,
-                                                         c->cnt, c->off, c->ckeys[0], c->cvals[0], c->d_state);
+  const vbx_ctx::ScratchSet& S = x.S;
+  k_rays_emit_warp<KeyT><<<x.sms * 8, 128, 0, x.s>>>(S.d_args, S.blocks, keys, S.ray_list, S.head_list, S.ray_p, S.cnt,
+                                                     S.off, S.ckeys[0], S.cvals[0], S.d_state);
 }
 
 // Stages up to the record offsets (for the Merged single walk also the trace that writes the update records):
 // everything that decides WHICH voxels are updated.  The per-scan values
-// come from the argument block (c->d_args), and the grids are sized for max_points_per_scan -- surplus threads
+// come from the set's argument block (S.d_args), and the grids are sized for max_points_per_scan -- surplus threads
 // exit at once -- so that one captured graph serves scans of any size (the point sort's grid, whose surplus
 // blocks would wait between passes, is set per scan instead: update_scan_graph).
 template <typename KeyT>
-static int front_half(vbx_ctx* c, const ScanParams& P, const uint32_t* order, Marks& mk, uint64_t* launches,
-                      const KeyT** keys_out) {
-  cudaStream_t s = c->stream;
-  const ScanArgs* A = c->d_args;
+static int front_half(vbx_ctx* c, const ScanRoute& x, const ScanParams& P, const uint32_t* order, Marks& mk,
+                      uint64_t* launches, const KeyT** keys_out) {
+  cudaStream_t s = x.s;
+  const vbx_ctx::ScratchSet& S = x.S;
+  const vbx_ctx::FrontLane& F = x.F;
+  const Tables tab = scan_tables(c, S);
+  const ScanArgs* A = S.d_args;
   const uint32_t n = P.n;
   const uint32_t gn = c->max_points;
   const int TB = 256;
@@ -2287,69 +2311,69 @@ static int front_half(vbx_ctx* c, const ScanParams& P, const uint32_t* order, Ma
   const uint32_t* scan_limit = nullptr;
   const uint32_t scan_tiles = (gn + 1 + kScanTile - 1) / kScanTile;
   if (P.kind == VBX_MERGED) {
-    KeyT* k0 = reinterpret_cast<KeyT*>(c->pkeys[0]);
-    KeyT* k1 = reinterpret_cast<KeyT*>(c->pkeys[1]);
-    k_point_bounds<<<std::min<unsigned int>(grid_for(gn, TB), c->grid_sms * 4), TB, 0, s>>>(
-        A, c->first_bits, c->sort_plan[0], c->scan_status, scan_tiles + 1, c->d_state);
-    k_point_keys<KeyT><<<grid_for(gn, TB), TB, 0, s>>>(A, order, k0, c->pvals[0], c->d_state);
+    KeyT* k0 = reinterpret_cast<KeyT*>(S.pkeys0);
+    KeyT* k1 = reinterpret_cast<KeyT*>(F.pkeys1);
+    k_point_bounds<<<std::min<unsigned int>(grid_for(gn, TB), x.sms * 4), TB, 0, s>>>(
+        A, F.first_bits, F.sort_plan0, F.scan_status, scan_tiles + 1, S.d_state);
+    k_point_keys<KeyT><<<grid_for(gn, TB), TB, 0, s>>>(A, order, k0, F.pvals[0], S.d_state);
     mk.mark(0);
     // the bits in use are known on the device only (ScanState::key_bits): passes beyond them exit at once
-    if (int rc = own_sort<KeyT>(c, 0, k0, c->pvals[0], k1, c->pvals[1], &A->n, 0, n, 8 * (int)sizeof(KeyT), true,
-                                launches, &c->d_state->key_bits, /*plan_cleared=*/true)) {
+    if (int rc = own_sort<KeyT>(c, x, 0, k0, F.pvals[0], k1, F.pvals[1], &A->n, 0, n, 8 * (int)sizeof(KeyT), true,
+                                launches, &S.d_state->key_bits, /*plan_cleared=*/true)) {
       return rc;
     }
     keys = k0;
-    vals = c->pvals[0];
+    vals = F.pvals[0];
     mk.mark(1);
-    k_heads<KeyT><<<grid_for((uint64_t)gn + 1, TB), TB, 0, s>>>(A, keys, vals, c->order_inv, c->head_list, c->big_list,
-                                                                c->first_bits, c->cnt, c->d_state);
+    k_heads<KeyT><<<grid_for((uint64_t)gn + 1, TB), TB, 0, s>>>(A, keys, vals, c->order_inv, S.head_list, F.big_list,
+                                                                F.first_bits, S.cnt, S.d_state);
     // The reference's bundle order (ray_list[rank] = bundle id, vbx_order.cuh) is one thread block's work
     // and the fold (k_merge) does not need it: the two run side by side.  (With stage profiling on they
     // run one after the other so that each gets its own time.)
-    cudaStream_t so = c->profiling ? s : c->side_stream;
+    cudaStream_t so = mk.on ? s : F.side;
     if (so != s) {
-      VBX_CUDA(c, cudaEventRecord(c->ev_fork, s));
-      VBX_CUDA(c, cudaStreamWaitEvent(so, c->ev_fork, 0));
+      VBX_CUDA(c, cudaEventRecord(F.ev_fork, s));
+      VBX_CUDA(c, cudaStreamWaitEvent(so, F.ev_fork, 0));
     }
-    if (int rc = launch_bundle_order<KeyT>(c, so, P.n, keys, vals)) return rc;
-    if (so != s) VBX_CUDA(c, cudaEventRecord(c->ev_join, so));
+    if (int rc = launch_bundle_order<KeyT>(c, x, so, P.n, keys, vals)) return rc;
+    if (so != s) VBX_CUDA(c, cudaEventRecord(F.ev_join, so));
     mk.mark(12);
-    k_merge<KeyT><<<c->grid_sms * 4, 192, 0, s>>>(A, keys, vals, c->head_list, c->big_list, c->ray_p, c->ray_a, c->ray_c,
-                                                  c->cnt, c->d_state);
+    k_merge<KeyT><<<x.sms * 4, 192, 0, s>>>(A, keys, vals, S.head_list, F.big_list, S.ray_p, S.ray_a, S.ray_c, S.cnt,
+                                            S.d_state);
     mk.mark(8);
     *launches += 8;
     if (!P.single_walk) {
       // the bundle count is only known on the device: launch for the worst case (every
       // point its own bundle); surplus threads exit on the first load
-      k_rays_count<KeyT><<<grid_for(gn, 128), 128, 0, s>>>(A, c->tab, order, keys, c->head_list, c->ray_p, c->ray_a,
-                                                           c->ray_c, c->cnt, c->set_start, c->set_observed, c->d_state);
+      k_rays_count<KeyT><<<grid_for(gn, 128), 128, 0, s>>>(A, tab, order, keys, S.head_list, S.ray_p, S.ray_a, S.ray_c,
+                                                           S.cnt, c->set_start, c->set_observed, S.d_state);
       *launches += 1;
     }
-    if (so != s) VBX_CUDA(c, cudaStreamWaitEvent(s, c->ev_join, 0));
+    if (so != s) VBX_CUDA(c, cudaStreamWaitEvent(s, F.ev_join, 0));
     // record offsets in RANK order: off[rank] = sum of cnt[ray_list[r]] over r < rank
-    scan_perm = c->ray_list;
-    scan_limit = &c->d_state->n_ray_list;
+    scan_perm = S.ray_list;
+    scan_limit = &S.d_state->n_ray_list;
   } else {
-    k_rays_count<KeyT><<<grid_for((uint64_t)gn + 1, 128), 128, 0, s>>>(A, c->tab, order, keys, c->head_list, c->ray_p,
-                                                                       c->ray_a, c->ray_c, c->cnt, c->set_start,
-                                                                       c->set_observed, c->d_state);
+    k_rays_count<KeyT><<<grid_for((uint64_t)gn + 1, 128), 128, 0, s>>>(A, tab, order, keys, S.head_list, S.ray_p, S.ray_a,
+                                                                       S.ray_c, S.cnt, c->set_start, c->set_observed,
+                                                                       S.d_state);
     *launches += 1;
   }
   mk.mark(2);
   {
     // record offsets; the scan's last position also settles the call's update count (total_found, total_updates,
     // kErrUpdatesFull: too many for one pass; nothing downstream runs on a call that failed)
-    if (P.kind != VBX_MERGED) VBX_CUDA(c, cudaMemsetAsync(c->scan_status, 0, (size_t)(scan_tiles + 1) * sizeof(uint32_t), s));  // (Merged: k_point_bounds did)
-    k_exclusive_scan<<<std::min<uint32_t>(scan_tiles, c->grid_sms * 4), kSortThreads, 0, s>>>(
-        c->cnt, scan_perm, scan_limit, c->off, &A->n_scan, 0u, c->scan_status + 1, c->scan_status, &c->d_state->total_found,
-        &c->d_state->total_updates, &c->d_state->error, (unsigned long long)c->max_updates, kErrUpdatesFull);
+    if (P.kind != VBX_MERGED) VBX_CUDA(c, cudaMemsetAsync(F.scan_status, 0, (size_t)(scan_tiles + 1) * sizeof(uint32_t), s));  // (Merged: k_point_bounds did)
+    k_exclusive_scan<<<std::min<uint32_t>(scan_tiles, x.sms * 4), kSortThreads, 0, s>>>(
+        S.cnt, scan_perm, scan_limit, S.off, &A->n_scan, 0u, F.scan_status + 1, F.scan_status, &S.d_state->total_found,
+        &S.d_state->total_updates, &S.d_state->error, (unsigned long long)c->max_updates, kErrUpdatesFull);
   }
   mk.mark(3);
   *launches += 1;
   if (traced_in_front(P)) {
     // the Merged trace needs nothing of the map: it ends the front half, so the walk stage (submission
     // order) is left with k_assign's block creation
-    launch_trace<KeyT>(c, keys, s);
+    launch_trace<KeyT>(x, keys);
     mk.mark(5);
     *launches += 1;
   }
@@ -2357,11 +2381,13 @@ static int front_half(vbx_ctx* c, const ScanParams& P, const uint32_t* order, Ma
   return VBX_OK;
 }
 
-// update-record sort + the apply kernels.  given: the records' values are ordinals into these arrays, not
-// ray ids (debug_apply)
-static int sort_and_apply(vbx_ctx* c, Marks& mk, uint64_t* launches, const GivenRecords* given = nullptr) {
-  cudaStream_t s = c->stream;
-  const vbx_ctx::Capture* cap = c->cap;
+// update-record sort + the apply kernels.  cap: a pipelined scan's graph is being captured.  given: the records'
+// values are ordinals into these arrays, not ray ids (debug_apply)
+static int sort_and_apply(vbx_ctx* c, const ScanRoute& x, Marks& mk, uint64_t* launches, const Capture* cap,
+                          const GivenRecords* given = nullptr) {
+  ScanRoute r = x;
+  const vbx_ctx::ScratchSet& S = x.S;
+  const Tables tab = scan_tables(c, S);
   RecordView rv;
   {
     // K and the number of touched blocks are only known on the device: sort on every bit a
@@ -2370,37 +2396,36 @@ static int sort_and_apply(vbx_ctx* c, Marks& mk, uint64_t* launches, const Given
     if (cap) {
       // pipelined submission: the record sort works on buffers private to this scan, so it leaves
       // the walk stream (which the next scan's ray walk is waiting for)
-      VBX_CUDA(c, cudaEventRecordWithFlags(cap->walked, s, cudaEventRecordExternal));
-      VBX_CUDA(c, cudaEventRecord(cap->edge[0], s));
+      VBX_CUDA(c, cudaEventRecordWithFlags(cap->walked, r.s, cudaEventRecordExternal));
+      VBX_CUDA(c, cudaEventRecord(cap->edge[0], r.s));
       VBX_CUDA(c, cudaStreamWaitEvent(cap->sort, cap->edge[0], 0));
       VBX_CUDA(c, cudaStreamWaitEvent(cap->sort, cap->prev_sorted, cudaEventWaitExternal));
-      s = cap->sort;
-      c->stream = s;
+      r.s = cap->sort;
     }
-    if (int rc = own_sort<uint32_t>(c, 1, c->ckeys[0], c->cvals[0], c->ckeys[1], c->cvals[1], &c->d_state->total_updates,
-                                     0, c->record_hint, key_bits, false, launches, &c->d_state->rec_key_bits,
+    if (int rc = own_sort<uint32_t>(c, r, 1, S.ckeys[0], S.cvals[0], S.ckeys[1], S.cvals[1], &S.d_state->total_updates,
+                                     0, c->record_hint, key_bits, false, launches, &S.d_state->rec_key_bits,
                                      /*plan_cleared=*/true)) {
       return rc;
     }
-    rv.keys[0] = c->ckeys[0];
-    rv.keys[1] = c->ckeys[1];
-    rv.vals[0] = c->cvals[0];
-    rv.vals[1] = c->cvals[1];
-    rv.plan = c->sort_plan[1];
-    rv.d_total = &c->d_state->total_updates;
+    rv.keys[0] = S.ckeys[0];
+    rv.keys[1] = S.ckeys[1];
+    rv.vals[0] = S.cvals[0];
+    rv.vals[1] = S.cvals[1];
+    rv.plan = S.sort_plan1;
+    rv.d_total = &S.d_state->total_updates;
     rv.total_fixed = 0;
   }
   LongRuns lr;
-  lr.start = c->long_list;
-  lr.end = c->long_end;
-  lr.keep = c->keep_bits;
+  lr.start = S.long_list;
+  lr.end = S.long_end;
+  lr.keep = S.keep_bits;
   lr.cap = c->max_updates / 32 + 1;
   // everything of the apply that does not depend on the map, on the (pipelined: scan-private) sort stream
+  cudaStream_t s = r.s;
   if (given) {
-    k_apply_prep<true><<<c->grid_sms * 8, 256, 0, s>>>(c->d_args, c->tab, rv, c->ray_a, c->ray_c, lr, c->d_state, *given);
+    k_apply_prep<true><<<x.sms * 8, 256, 0, s>>>(S.d_args, tab, rv, S.ray_a, S.ray_c, lr, S.d_state, *given);
   } else {
-    k_apply_prep<false><<<c->grid_sms * 8, 256, 0, s>>>(c->d_args, c->tab, rv, c->ray_a, c->ray_c, lr, c->d_state,
-                                                        GivenRecords{});
+    k_apply_prep<false><<<x.sms * 8, 256, 0, s>>>(S.d_args, tab, rv, S.ray_a, S.ray_c, lr, S.d_state, GivenRecords{});
   }
   mk.mark(6);
   if (cap) {
@@ -2412,7 +2437,7 @@ static int sort_and_apply(vbx_ctx* c, Marks& mk, uint64_t* launches, const Given
     VBX_CUDA(c, cudaStreamWaitEvent(cap->apply, cap->prev_applied, cudaEventWaitExternal));
     s = cap->apply;
   }
-  k_apply<<<c->grid_sms * 8, 32 * kApplyWarps, 0, s>>>(c->d_args, c->tab, rv, lr, c->d_state);
+  k_apply<<<x.sms * 8, 32 * kApplyWarps, 0, s>>>(S.d_args, tab, rv, lr, S.d_state);
   if (cap) VBX_CUDA(c, cudaEventRecordWithFlags(cap->applied, s, cudaEventRecordExternal));
   mk.mark(7);
   *launches += 2;
@@ -2422,24 +2447,26 @@ static int sort_and_apply(vbx_ctx* c, Marks& mk, uint64_t* launches, const Given
 // emitted: the front half has already written this call's update records (traced_in_front, one pass); the
 // passes of apply_in_passes trace their own rank window here.
 template <typename KeyT>
-static int back_half(vbx_ctx* c, const ScanParams& P, const KeyT* keys, bool emitted, Marks& mk, uint64_t* launches) {
-  cudaStream_t s = c->stream;
+static int back_half(vbx_ctx* c, const ScanRoute& x, const ScanParams& P, const KeyT* keys, bool emitted, Marks& mk,
+                     uint64_t* launches, const Capture* cap = nullptr) {
+  cudaStream_t s = x.s;
+  const vbx_ctx::ScratchSet& S = x.S;
+  const Tables tab = scan_tables(c, S);
   if (!emitted) {
     if (traced_in_front(P)) {
-      launch_trace<KeyT>(c, keys, s);
+      launch_trace<KeyT>(x, keys);
     } else {
-      k_rays_emit<KeyT><<<grid_for(c->max_points, 128), 128, 0, s>>>(c->d_args, c->tab, keys, c->ray_list, c->head_list,
-                                                                     c->ray_p, c->cnt, c->off, c->ckeys[0], c->cvals[0],
-                                                                     c->d_state);
+      k_rays_emit<KeyT><<<grid_for(c->max_points, 128), 128, 0, s>>>(S.d_args, tab, keys, S.ray_list, S.head_list, S.ray_p,
+                                                                     S.cnt, S.off, S.ckeys[0], S.cvals[0], S.d_state);
     }
     mk.mark(5);
     *launches += 1;
   }
-  k_assign<<<1, kAssignThreads, 0, s>>>(c->tab, c->blocks, c->d_args, c->d_nblocks, c->sort_plan[1], c->d_state);
+  k_assign<<<1, kAssignThreads, 0, s>>>(tab, S.blocks, S.d_args, c->d_nblocks, S.sort_plan1, S.d_state);
   c->nb_cur ^= 1;
   mk.mark(4);
   *launches += 1;
-  return sort_and_apply(c, mk, launches);
+  return sort_and_apply(c, x, mk, launches, cap);
 }
 
 static void fill_args(const vbx_ctx* c, const ScanParams& P, const float* xyz, const uint8_t* rgba, ScanArgs* a) {
@@ -2452,11 +2479,11 @@ static void fill_args(const vbx_ctx* c, const ScanParams& P, const float* xyz, c
   a->count_paths = c->count_apply_paths ? 1u : 0u;
 }
 
-// The synchronous calls' argument block goes through hand-off set 0's page-locked copy: the host writes it
+// The synchronous calls' argument block goes through the set's page-locked copy: the host writes it
 // only when the stream has finished every earlier upload.
-static int upload_args(vbx_ctx* c, const ScanArgs& a) {
-  *c->h_args = a;
-  VBX_CUDA(c, cudaMemcpyAsync(c->d_args, c->h_args, sizeof(ScanArgs), cudaMemcpyHostToDevice, c->stream));
+static int upload_args(vbx_ctx* c, const ScanRoute& x, const ScanArgs& a) {
+  *x.S.h_args = a;
+  VBX_CUDA(c, cudaMemcpyAsync(x.S.d_args, x.S.h_args, sizeof(ScanArgs), cudaMemcpyHostToDevice, x.s));
   return VBX_OK;
 }
 
@@ -2468,15 +2495,15 @@ int alloc_scan_args(vbx_ctx* c, vbx_ctx::ScratchSet& S) {
 
 // The back half of a call whose K exceeds max_updates_per_pass, in passes (see integrate_device).
 template <typename KeyT>
-static int apply_in_passes(vbx_ctx* c, ScanArgs a, const KeyT* keys, Marks& mk, uint64_t* launches) {
-  cudaStream_t s = c->stream;
+static int apply_in_passes(vbx_ctx* c, const ScanRoute& x, ScanArgs a, const KeyT* keys, Marks& mk, uint64_t* launches) {
+  cudaStream_t s = x.s;
   const uint32_t n = a.P.n;
   std::vector<uint32_t> off(n + 1);
-  VBX_CUDA(c, cudaMemcpyAsync(off.data(), c->off, (size_t)(n + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(off.data(), x.S.off, (size_t)(n + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));
   if (a.P.kind == VBX_MERGED) {
     // the scan wrote the offsets of the bundles and, at [n], the total; ranks past the last bundle hold nothing
-    const uint32_t nr = std::min(c->h_state->n_ray_list, n);
+    const uint32_t nr = std::min(x.S.h_state->n_ray_list, n);
     for (uint32_t i = nr + 1; i < n; ++i) off[i] = off[n];
   }
   // every pass's slot range first: a call that cannot be split is refused before any pass runs (the Merged
@@ -2502,10 +2529,10 @@ static int apply_in_passes(vbx_ctx* c, ScanArgs a, const KeyT* keys, Marks& mk, 
     a.P.emit_base = off[lo];
     a.nb_cur = (uint32_t)c->nb_cur;
     VBX_CUDA(c, cudaStreamSynchronize(s));  // (the previous pass has read its arguments)
-    if (int rc = upload_args(c, a)) return rc;
-    k_pass_begin<<<1, 1, 0, s>>>(c->d_state, kp);
+    if (int rc = upload_args(c, x, a)) return rc;
+    k_pass_begin<<<1, 1, 0, s>>>(x.S.d_state, kp);
     *launches += 1;
-    if (int rc = back_half<KeyT>(c, a.P, keys, /*emitted=*/false, mk, launches)) return rc;
+    if (int rc = back_half<KeyT>(c, x, a.P, keys, /*emitted=*/false, mk, launches)) return rc;
     ++passes;
   }
   c->last_passes = passes;
@@ -2564,12 +2591,14 @@ static void fill_params(vbx_ctx* c, int kind, const float q[4], const float t[3]
   P.single_walk = (kind != VBX_FAST && !(kind == VBX_MERGED && cfg.enable_anti_grazing)) ? 1 : 0;
 }
 
-int integrate_device(vbx_ctx* c, int kind, const float q[4], const float t[3], const float* d_xyz,
+int integrate_device(vbx_ctx* c, const ScanRoute& x, int kind, const float q[4], const float t[3], const float* d_xyz,
                      const uint8_t* d_rgba, uint64_t n64, int freespace) {
   if (kind < VBX_SIMPLE || kind > VBX_FAST) return fail(c, VBX_E_INVALID, "Unknown TSDF integrator type");
   if (n64 > c->max_points) return fail(c, VBX_E_CAPACITY, "cloud larger than max_points_per_scan");
   const uint32_t n = (uint32_t)n64;
-  cudaStream_t s = c->stream;
+  cudaStream_t s = x.s;
+  const vbx_ctx::ScratchSet& S = x.S;
+  const vbx_ctx::FrontLane& F = x.F;
   const vbx_tsdf_config& cfg = c->cfg;
   std::memset(c->counters, 0, sizeof(c->counters));
   uint64_t launches = 0;
@@ -2578,7 +2607,7 @@ int integrate_device(vbx_ctx* c, int kind, const float q[4], const float t[3], c
   fill_params(c, kind, q, t, n, freespace, P);
 
   VBX_CUDA(c, cudaEventRecord(c->ev0, s));
-  VBX_CUDA(c, cudaMemsetAsync(c->d_state, 0, sizeof(ScanState), s));
+  VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), s));
   if (n == 0) {
     VBX_CUDA(c, cudaEventRecord(c->ev1, s));
     VBX_CUDA(c, cudaStreamSynchronize(s));
@@ -2587,78 +2616,66 @@ int integrate_device(vbx_ctx* c, int kind, const float q[4], const float t[3], c
   }
   ScanArgs a;
   fill_args(c, P, d_xyz, d_rgba, &a);
-  if (int rc = upload_args(c, a)) return rc;
+  if (int rc = upload_args(c, x, a)) return rc;
   const int TB = 256;
-  Marks mk;
-  mk.c = c;
-  mk.s = s;
+  Marks mk{c, s, x.marks};
   mk.begin();
 
   const uint32_t* order = nullptr;
   if (cfg.integration_order_mode == 1) {
     // SortedThreadSafeIndex: ascending |p|^2 (stable here; std::sort leaves ties unspecified)
-    k_sqnorm_keys<<<grid_for(n, TB), TB, 0, s>>>(n, d_xyz, c->pkeys[0], c->pvals[0]);
-    if (int rc = own_sort<uint64_t>(c, 0, c->pkeys[0], c->pvals[0], c->pkeys[1], c->pvals[1], nullptr, n, n, 64, true, &launches)) {
+    k_sqnorm_keys<<<grid_for(n, TB), TB, 0, s>>>(n, d_xyz, S.pkeys0, F.pvals[0]);
+    if (int rc = own_sort<uint64_t>(c, x, 0, S.pkeys0, F.pvals[0], F.pkeys1, F.pvals[1], nullptr, n, n, 64, true, &launches)) {
       return rc;
     }
-    VBX_CUDA(c, cudaMemcpyAsync(c->order, c->pvals[0], n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+    VBX_CUDA(c, cudaMemcpyAsync(c->order, F.pvals[0], n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
     k_invert_order<<<grid_for(n, TB), TB, 0, s>>>(n, c->order, c->order_inv);
     order = c->order;
     launches += 2;
   }
 
-  uint32_t chunk_blocks_before = 0;
-  bool chunked = false;
   const uint64_t* keys64 = nullptr;
-  unsigned long long K = 0;
-  uint32_t n_touched = 0;
-  if (int rc = front_half<uint64_t>(c, P, order, mk, &launches, &keys64)) return rc;
-  {
-    // own sort: K stays on the device, the whole call is enqueued without a host round trip
-    if (int rc = back_half<uint64_t>(c, P, keys64, traced_in_front(P), mk, &launches)) return rc;
-    VBX_CUDA(c, cudaEventRecord(c->ev1, s));
-    VBX_CUDA(c, cudaMemcpyAsync(c->h_state, c->d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
-    VBX_CUDA(c, cudaStreamSynchronize(s));
-    if (c->h_state->error == kErrUpdatesFull) {
-      // More update records than one pass holds.  Nothing was emitted or applied; the per-ray
-      // tables, counts and offsets of the front half stand.  Apply the call in passes over
-      // contiguous ray-slot ranges: every voxel still sees its updates in ray-rank order, so
-      // the result is the one-pass result bit for bit.
-      chunk_blocks_before = c->n_blocks;
-      if (int rc = apply_in_passes<uint64_t>(c, a, keys64, mk, &launches)) return rc;
-      chunked = true;
-      VBX_CUDA(c, cudaEventRecord(c->ev1, s));
-      VBX_CUDA(c, cudaMemcpyAsync(c->h_state, c->d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
-      VBX_CUDA(c, cudaStreamSynchronize(s));
-    }
-    if (int rc = check_state_errors(c, c->h_state->error)) return rc;
-    c->n_blocks = c->h_state->n_blocks;
-    K = c->h_state->total_found;
-    n_touched = c->h_state->n_touched;
-  }
+  if (int rc = front_half<uint64_t>(c, x, P, order, mk, &launches, &keys64)) return rc;
+  // own sort: K stays on the device, the whole call is enqueued without a host round trip
+  if (int rc = back_half<uint64_t>(c, x, P, keys64, traced_in_front(P), mk, &launches)) return rc;
   VBX_CUDA(c, cudaEventRecord(c->ev1, s));
-  VBX_CUDA(c, cudaMemcpyAsync(c->h_state, c->d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));
+  const ScanState& h = *S.h_state;
+  const uint32_t blocks_before = c->n_blocks;
+  const bool chunked = h.error == kErrUpdatesFull;
+  if (chunked) {
+    // More update records than one pass holds.  Nothing was emitted or applied; the per-ray
+    // tables, counts and offsets of the front half stand.  Apply the call in passes over
+    // contiguous ray-slot ranges: every voxel still sees its updates in ray-rank order, so
+    // the result is the one-pass result bit for bit.
+    if (int rc = apply_in_passes<uint64_t>(c, x, a, keys64, mk, &launches)) return rc;
+    VBX_CUDA(c, cudaEventRecord(c->ev1, s));
+    VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+    VBX_CUDA(c, cudaStreamSynchronize(s));
+  }
+  if (int rc = check_state_errors(c, h)) return rc;
+  c->n_blocks = h.n_blocks;
+  const unsigned long long K = h.total_found;
   VBX_CUDA(c, cudaGetLastError());
   VBX_CUDA(c, cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   mk.collect();
   c->launches += launches;
-  c->counters[0] = c->h_state->n_rays;
-  if (kind == VBX_MERGED) c->bundle_hint = std::max(c->h_state->n_rays, c->h_state->n_clear_rays);
-  c->counters[1] = c->h_state->n_clear_rays;
+  c->counters[0] = h.n_rays;
+  if (kind == VBX_MERGED) c->bundle_hint = std::max(h.n_rays, h.n_clear_rays);
+  c->counters[1] = h.n_clear_rays;
   c->counters[2] = K;
   if (K) c->record_hint = K;
-  c->counters[3] = c->h_state->n_voxels;
-  c->counters[4] = n_touched;
-  c->counters[5] = chunked ? (uint64_t)(c->n_blocks - chunk_blocks_before) : (uint64_t)c->h_state->n_new;
+  c->counters[3] = h.n_voxels;
+  c->counters[4] = h.n_touched;
+  c->counters[5] = chunked ? (uint64_t)(c->n_blocks - blocks_before) : (uint64_t)h.n_new;
   c->counters[11] = chunked ? c->last_passes : 1;
-  c->counters[9] = c->h_state->n_refold;
-  c->counters[10] = c->h_state->refold_members;
-  c->counters[12] = c->h_state->key_bits;
-  c->counters[6] = (kind == VBX_MERGED) ? c->h_state->n_valid_points
-                                        : (uint64_t)c->h_state->n_rays + c->h_state->n_clear_rays;
+  c->counters[9] = h.n_refold;
+  c->counters[10] = h.refold_members;
+  c->counters[12] = h.key_bits;
+  c->counters[6] = (kind == VBX_MERGED) ? h.n_valid_points : (uint64_t)h.n_rays + h.n_clear_rays;
   c->counters[7] = launches;
-  for (int i = 0; i < kApplyPaths; ++i) c->apply_paths[i] = c->h_state->apply_paths[i];
+  for (int i = 0; i < kApplyPaths; ++i) c->apply_paths[i] = h.apply_paths[i];
   return VBX_OK;
 }
 
@@ -2685,18 +2702,18 @@ int integrate_device(vbx_ctx* c, int kind, const float q[4], const float t[3], c
 // the previous scan's walk, the record sort for the one two scans back, the apply for the previous
 // scan's apply.  An event-record node of an earlier launched graph is the event's most recent record
 // for a later one (tests/test_async_graph_gpu.py checks the maps bit for bit against synchronous calls).
+// sms: the grid unit of the graph's kernels.
 static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& F, const ScanParams& P,
-                        vbx_ctx::ScanGraph& G) {
+                        vbx_ctx::ScanGraph& G, unsigned int sms) {
   const int k = (int)(&S - c->set), sets = c->sets_in_use;
   const vbx_ctx::ScratchSet& prev = c->set[(k + sets - 1) % sets];
   const vbx_ctx::ScratchSet& prev2 = c->set[(k + 2 * sets - 2) % sets];
-  const vbx_ctx::Capture cap{c->stream_s, c->stream_main, S.walked, S.sorted, S.applied, prev2.sorted, prev.applied,
-                             {c->cap_ev[2], c->cap_ev[3]}};
+  const Capture cap{c->stream_s, c->stream, S.walked, S.sorted, S.applied, prev2.sorted, prev.applied,
+                    {c->cap_ev[2], c->cap_ev[3]}};
+  const ScanRoute front{S, F, F.stream, sms, false}, walk{S, F, c->stream_e, sms, false};
   cudaStream_t o = S.stream;
   uint64_t launches = 0;
-  Marks mk;  // (stage profiling is off while a graph is captured)
-  mk.c = c;
-  mk.s = F.stream;
+  Marks mk{c, F.stream, false};
   auto enqueue = [&]() -> int {
     VBX_CUDA(c, cudaMemcpyAsync(S.d_args, S.h_args, sizeof(ScanArgs), cudaMemcpyHostToDevice, o));
     VBX_CUDA(c, cudaStreamWaitEvent(o, S.copy_done, cudaEventWaitExternal));  // a host cloud's copy
@@ -2704,29 +2721,26 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
     // ---- front half on the lane's stream
     VBX_CUDA(c, cudaEventRecord(c->cap_ev[0], o));
     VBX_CUDA(c, cudaStreamWaitEvent(F.stream, c->cap_ev[0], 0));
-    c->stream = F.stream;
     VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), F.stream));
     if (c->timeline) VBX_CUDA(c, cudaEventRecordWithFlags(S.front_start, F.stream, cudaEventRecordExternal));
     const uint64_t* keys64 = nullptr;
-    if (int rc = front_half<uint64_t>(c, P, nullptr, mk, &launches, &keys64)) return rc;
+    if (int rc = front_half<uint64_t>(c, front, P, nullptr, mk, &launches, &keys64)) return rc;
     VBX_CUDA(c, cudaEventRecordWithFlags(F.done, F.stream, cudaEventRecordExternal));
     if (c->timeline) VBX_CUDA(c, cudaEventRecordWithFlags(S.front_done, F.stream, cudaEventRecordExternal));
     // ---- walk, record sort and apply (sort_and_apply hands off between their streams)
     VBX_CUDA(c, cudaEventRecord(c->cap_ev[1], F.stream));
     VBX_CUDA(c, cudaStreamWaitEvent(c->stream_e, c->cap_ev[1], 0));
     VBX_CUDA(c, cudaStreamWaitEvent(c->stream_e, prev.walked, cudaEventWaitExternal));
-    c->stream = c->stream_e;
-    c->cap = &cap;
     // Scans run their map-touching stages in submission order.  A scan that cannot be applied
     // asynchronously (more update records than one pass holds) raises the context's hold flag here;
     // every scan queued behind it then skips its back half, and the host redoes all of them
     // synchronously, in order, from the retained inputs (recover_async, vbx_capi.cu).
     k_back_begin<<<1, 1, 0, c->stream_e>>>(S.d_state, c->d_hold);
     launches += 1;
-    if (int rc = back_half<uint64_t>(c, P, keys64, traced_in_front(P), mk, &launches)) return rc;
+    if (int rc = back_half<uint64_t>(c, walk, P, keys64, traced_in_front(P), mk, &launches, &cap)) return rc;
     VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, cap.apply));
     // every stream of the capture joins its origin
-    const cudaStream_t joined[4] = {F.stream, c->stream_e, c->stream_s, c->stream_main};
+    const cudaStream_t joined[4] = {F.stream, c->stream_e, c->stream_s, c->stream};
     for (int j = 0; j < 4; ++j) {
       VBX_CUDA(c, cudaEventRecord(c->cap_ev[4 + j], joined[j]));
       VBX_CUDA(c, cudaStreamWaitEvent(o, c->cap_ev[4 + j], 0));
@@ -2737,8 +2751,6 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
   int rc = enqueue();
   cudaGraph_t g = nullptr;
   const cudaError_t e = cudaStreamEndCapture(o, &g);
-  c->cap = nullptr;
-  c->stream = c->stream_main;
   if (rc == VBX_OK && e != cudaSuccess) rc = cuda_fail(c, e, "cudaStreamEndCapture");
   // Per-node stage priorities (apply > walk > sort > front, as the streams of the unpipelined stages had)
   // and the nodes whose launch shape follows the scan or the hints.
@@ -2825,12 +2837,12 @@ static int set_grid(vbx_ctx* c, vbx_ctx::ScanGraph& G, cudaGraphNode_t node, uns
 
 // Brings the kernel nodes of a scan graph whose launch shape varies up to date (a no-op unless it moved):
 // the point sort's grid (a grid larger than the scan's tiles keeps blocks waiting between passes), the
-// record sort's grid, k_bundle_order's form (grid) and shared memory.
-static int update_scan_graph(vbx_ctx* c, vbx_ctx::ScanGraph& G, uint32_t n) {
+// record sort's grid, k_bundle_order's form (grid) and shared memory.  sms: the grid unit the graph was captured with.
+static int update_scan_graph(vbx_ctx* c, vbx_ctx::ScanGraph& G, uint32_t n, unsigned int sms) {
   if (G.point_sort) {
-    if (int rc = set_grid(c, G, G.point_sort, sort_grid(c, 0, n), &G.point_grid)) return rc;
+    if (int rc = set_grid(c, G, G.point_sort, sort_grid(c, 0, n, sms), &G.point_grid)) return rc;
   }
-  if (int rc = set_grid(c, G, G.record_sort, sort_grid(c, 1, c->record_hint), &G.record_grid)) return rc;
+  if (int rc = set_grid(c, G, G.record_sort, sort_grid(c, 1, c->record_hint, sms), &G.record_grid)) return rc;
   if (G.order) {
     const OrderLaunch o = order_launch(c, n);
     if (o.grid != G.order_grid || o.smem_bytes != G.order_smem) {
@@ -2851,8 +2863,10 @@ static int update_scan_graph(vbx_ctx* c, vbx_ctx::ScanGraph& G, uint32_t n) {
   return VBX_OK;
 }
 
-int integrate_async(vbx_ctx* c, int kind, const float q[4], const float t[3], const float* xyz, const uint8_t* rgba,
-                    uint64_t n64, int freespace, int on_device) {
+// sync: where a synchronous call goes (sync_route): the fallback for scans that cannot be overlapped, and the
+// grid unit the graphs' share of the GPU is taken from.
+int integrate_async(vbx_ctx* c, const ScanRoute& sync, int kind, const float q[4], const float t[3], const float* xyz,
+                    const uint8_t* rgba, uint64_t n64, int freespace, int on_device) {
   if (kind < VBX_SIMPLE || kind > VBX_FAST) return fail(c, VBX_E_INVALID, "Unknown TSDF integrator type");
   if (n64 > c->max_points) return fail(c, VBX_E_CAPACITY, "cloud larger than max_points_per_scan");
   const vbx_tsdf_config& cfg = c->cfg;
@@ -2864,12 +2878,12 @@ int integrate_async(vbx_ctx* c, int kind, const float q[4], const float t[3], co
     const float* dx = xyz;
     const uint8_t* dr = rgba;
     if (!on_device && n64) {
-      VBX_CUDA(c, cudaMemcpyAsync(c->d_xyz, xyz, n64 * 3 * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-      VBX_CUDA(c, cudaMemcpyAsync(c->d_rgba, rgba, n64 * 4, cudaMemcpyHostToDevice, c->stream));
-      dx = c->d_xyz;
-      dr = c->d_rgba;
+      VBX_CUDA(c, cudaMemcpyAsync(sync.S.d_xyz, xyz, n64 * 3 * sizeof(float), cudaMemcpyHostToDevice, sync.s));
+      VBX_CUDA(c, cudaMemcpyAsync(sync.S.d_rgba, rgba, n64 * 4, cudaMemcpyHostToDevice, sync.s));
+      dx = sync.S.d_xyz;
+      dr = sync.S.d_rgba;
     }
-    return integrate_device(c, kind, q, t, dx, dr, n64, freespace);
+    return integrate_device(c, sync, kind, q, t, dx, dr, n64, freespace);
   }
   if (int rc = ensure_async(c)) return rc;
   const uint32_t n = (uint32_t)n64;
@@ -2886,8 +2900,6 @@ int integrate_async(vbx_ctx* c, int kind, const float q[4], const float t[3], co
       if (int rc = drain_async(c)) return rc;
     }
   }
-  select_set(c, k);
-  select_lane(c, l);
   ScanParams P;
   fill_params(c, kind, q, t, n, freespace, P);
   const float* dx = xyz;
@@ -2913,26 +2925,17 @@ int integrate_async(vbx_ctx* c, int kind, const float q[4], const float t[3], co
   // The pipeline runs the kernels of several scans at once (front halves, a walk, a record sort, an apply):
   // a persistent grid sized for the whole GPU only holds SM slots that the other scans' kernels need.  The
   // graphs' grids are sized for a quarter of the SMs (DESIGN.md §5b: the pace against the grid scale).
-  const unsigned int full_sms = c->grid_sms;
-  c->grid_sms = std::max(1u, full_sms / 4);
+  const unsigned int sms = std::max(1u, sync.sms / 4);
   if (!G.exec) {
     // the first scan of its kind captures the graphs of every (set, lane) pair the submission order
     // reaches (set = seq % sets, lane = seq % lanes), so that no later scan waits for a capture
-    const bool profiling = c->profiling;
-    c->profiling = false;  // stage events would serialise the streams
     const int pairs = std::lcm(c->sets_in_use, c->lanes_in_use);
     for (int j = 0; j < pairs && rc == VBX_OK; ++j) {
       const int kj = j % c->sets_in_use, lj = j % c->lanes_in_use;
-      select_set(c, kj);
-      select_lane(c, lj);
-      rc = capture_scan(c, c->set[kj], c->lane[lj], P, c->set[kj].graph[lj][variant]);
+      rc = capture_scan(c, c->set[kj], c->lane[lj], P, c->set[kj].graph[lj][variant], sms);
     }
-    select_set(c, k);
-    select_lane(c, l);
-    c->profiling = profiling;
   }
-  if (rc == VBX_OK) rc = update_scan_graph(c, G, n);
-  c->grid_sms = full_sms;
+  if (rc == VBX_OK) rc = update_scan_graph(c, G, n, sms);
   if (rc == VBX_OK && (cudaGraphLaunch(G.exec, S.stream) != cudaSuccess || cudaEventRecord(S.back_done, S.stream) != cudaSuccess)) {
     rc = fail(c, VBX_E_CUDA, "launching the scan's graph failed");
   }
@@ -2976,25 +2979,26 @@ __global__ void k_debug_order_setup(OrderScratch g, uint32_t n, ScanState* st) {
 
 int debug_bundle_order(vbx_ctx* c, const uint32_t* hashes, uint32_t n, int force_global, uint32_t* out) {
   cudaStream_t s = c->stream;
+  const vbx_ctx::ScratchSet& S = c->set[0];
   if (n > c->max_points) return fail(c, VBX_E_CAPACITY, "debug_bundle_order: n > max_points_per_scan");
   if (n == 0) return VBX_OK;
-  VBX_CUDA(c, cudaMemsetAsync(c->d_state, 0, sizeof(ScanState), s));
-  VBX_CUDA(c, cudaMemcpyAsync(c->order_scratch.h, hashes, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-  k_debug_order_setup<<<grid_for(n, 256), 256, 0, s>>>(c->order_scratch, n, c->d_state);
   RehashSchedule rs = c->rehash;
-  OrderScratch g = c->order_scratch;
+  OrderScratch g = c->lane[0].order_scratch;
+  VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), s));
+  VBX_CUDA(c, cudaMemcpyAsync(g.h, hashes, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  k_debug_order_setup<<<grid_for(n, 256), 256, 0, s>>>(g, n, S.d_state);
   uint32_t smem_words = force_global ? 0u : (uint32_t)(c->order_smem_bytes / 4);
-  uint32_t* ray_list = c->ray_list;
-  uint32_t* cta_tot = c->order_scratch.cta_tot;
-  ScanState* st = c->d_state;
+  uint32_t* ray_list = S.ray_list;
+  uint32_t* cta_tot = g.cta_tot;
+  ScanState* st = S.d_state;
   void* args[] = {&rs, &g, &smem_words, &ray_list, &cta_tot, &st};
   VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_bundle_order, dim3(kOrderGrid), dim3(kOrderThreads), args,
                                           c->order_smem_bytes, s));
-  VBX_CUDA(c, cudaMemcpyAsync(out, c->ray_list, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-  VBX_CUDA(c, cudaMemcpyAsync(c->h_state, c->d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(out, S.ray_list, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));
   VBX_CUDA(c, cudaGetLastError());
-  if (c->h_state->error) return fail(c, VBX_E_CAPACITY, "debug_bundle_order: table capacity");
+  if (S.h_state->error) return fail(c, VBX_E_CAPACITY, "debug_bundle_order: table capacity");
   return VBX_OK;
 }
 
@@ -3007,31 +3011,34 @@ __global__ void k_iota(uint32_t* v, uint32_t n) {
 // record buffers with the count in device memory, 8 the point-key buffers with a host count.
 int debug_sort(vbx_ctx* c, const void* keys, int key_bytes, uint32_t n, int key_bits, void* keys_out,
                uint32_t* vals_out) {
-  cudaStream_t s = c->stream;
+  const ScanRoute x = sync_route(c);
+  const vbx_ctx::ScratchSet& S = x.S;
+  const vbx_ctx::FrontLane& F = x.F;
+  cudaStream_t s = x.s;
   uint64_t launches = 0;
   if (key_bytes == 4) {
     if (n > c->max_updates) return fail(c, VBX_E_CAPACITY, "debug_sort: n > max_updates_per_pass");
-    VBX_CUDA(c, cudaMemcpyAsync(c->ckeys[0], keys, (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    k_iota<<<c->grid_sms, 256, 0, s>>>(c->cvals[0], n);
-    VBX_CUDA(c, cudaMemsetAsync(c->d_state, 0, sizeof(ScanState), s));
+    VBX_CUDA(c, cudaMemcpyAsync(S.ckeys[0], keys, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    k_iota<<<c->grid_sms, 256, 0, s>>>(S.cvals[0], n);
+    VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), s));
     const unsigned long long nn = n;
-    VBX_CUDA(c, cudaMemcpyAsync(&c->d_state->total_updates, &nn, sizeof(nn), cudaMemcpyHostToDevice, s));
-    if (int rc = own_sort<uint32_t>(c, 1, c->ckeys[0], c->cvals[0], c->ckeys[1], c->cvals[1],
-                                     &c->d_state->total_updates, 0, n, key_bits, true, &launches)) {
+    VBX_CUDA(c, cudaMemcpyAsync(&S.d_state->total_updates, &nn, sizeof(nn), cudaMemcpyHostToDevice, s));
+    if (int rc = own_sort<uint32_t>(c, x, 1, S.ckeys[0], S.cvals[0], S.ckeys[1], S.cvals[1], &S.d_state->total_updates,
+                                     0, n, key_bits, true, &launches)) {
       return rc;
     }
-    VBX_CUDA(c, cudaMemcpyAsync(keys_out, c->ckeys[0], (size_t)n * 4, cudaMemcpyDeviceToHost, s));
-    VBX_CUDA(c, cudaMemcpyAsync(vals_out, c->cvals[0], (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+    VBX_CUDA(c, cudaMemcpyAsync(keys_out, S.ckeys[0], (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+    VBX_CUDA(c, cudaMemcpyAsync(vals_out, S.cvals[0], (size_t)n * 4, cudaMemcpyDeviceToHost, s));
   } else if (key_bytes == 8) {
     if (n > c->max_points) return fail(c, VBX_E_CAPACITY, "debug_sort: n > max_points_per_scan");
-    VBX_CUDA(c, cudaMemcpyAsync(c->pkeys[0], keys, (size_t)n * 8, cudaMemcpyHostToDevice, s));
-    k_iota<<<c->grid_sms, 256, 0, s>>>(c->pvals[0], n);
-    if (int rc = own_sort<uint64_t>(c, 0, c->pkeys[0], c->pvals[0], c->pkeys[1], c->pvals[1], nullptr, n, n, key_bits, true,
+    VBX_CUDA(c, cudaMemcpyAsync(S.pkeys0, keys, (size_t)n * 8, cudaMemcpyHostToDevice, s));
+    k_iota<<<c->grid_sms, 256, 0, s>>>(F.pvals[0], n);
+    if (int rc = own_sort<uint64_t>(c, x, 0, S.pkeys0, F.pvals[0], F.pkeys1, F.pvals[1], nullptr, n, n, key_bits, true,
                                      &launches)) {
       return rc;
     }
-    VBX_CUDA(c, cudaMemcpyAsync(keys_out, c->pkeys[0], (size_t)n * 8, cudaMemcpyDeviceToHost, s));
-    VBX_CUDA(c, cudaMemcpyAsync(vals_out, c->pvals[0], (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+    VBX_CUDA(c, cudaMemcpyAsync(keys_out, S.pkeys0, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
+    VBX_CUDA(c, cudaMemcpyAsync(vals_out, F.pvals[0], (size_t)n * 4, cudaMemcpyDeviceToHost, s));
   } else {
     return fail(c, VBX_E_INVALID, "debug_sort: key_bytes must be 4 or 8");
   }
@@ -3071,7 +3078,9 @@ __global__ void k_debug_apply_setup(Tables tab, const uint64_t* __restrict__ bke
 // Records of one voxel are applied in the order given.  Block updated() bits are left alone.
 int debug_apply(vbx_ctx* c, const int32_t* idx3, uint32_t nb, uint64_t n, const uint32_t* rec_block,
                 const uint32_t* rec_voxel, const float* sdf, const float* w, const uint8_t* rgba, uint64_t paths[16]) {
-  cudaStream_t s = c->stream;
+  const ScanRoute x = sync_route(c);
+  const vbx_ctx::ScratchSet& S = x.S;
+  cudaStream_t s = x.s;
   if (n > c->max_updates) return fail(c, VBX_E_INVALID, "debug_apply: more records than max_updates_per_pass");
   if (nb > c->tab.touched_cap) return fail(c, VBX_E_INVALID, "debug_apply: too many blocks");
   for (uint64_t r = 0; r < n; ++r) {
@@ -3114,29 +3123,27 @@ int debug_apply(vbx_ctx* c, const int32_t* idx3, uint32_t nb, uint64_t n, const 
     ScanArgs a;
     fill_args(c, P, nullptr, nullptr, &a);
     a.count_paths = 1u;
-    if (int rc = upload_args(c, a)) return rc;
-    VBX_CUDA(c, cudaMemsetAsync(c->d_state, 0, sizeof(ScanState), s));
-    VBX_CUDA(c, cudaMemsetAsync(c->sort_plan[1], 0, sizeof(SortPlan), s));  // (sort_and_apply expects it cleared)
+    if (int rc = upload_args(c, x, a)) return rc;
+    VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), s));
+    VBX_CUDA(c, cudaMemsetAsync(S.sort_plan1, 0, sizeof(SortPlan), s));  // (sort_and_apply expects it cleared)
     const uint64_t m = std::max<uint64_t>(n, nb);
     if (m) {
-      k_debug_apply_setup<<<grid_for(m, 256), 256, 0, s>>>(c->tab, d_bkeys, nb, d_block, d_voxel, n, c->L, c->ckeys[0],
-                                                           c->cvals[0], c->d_state, d_bad);
+      k_debug_apply_setup<<<grid_for(m, 256), 256, 0, s>>>(scan_tables(c, S), d_bkeys, nb, d_block, d_voxel, n, c->L,
+                                                           S.ckeys[0], S.cvals[0], S.d_state, d_bad);
     }
     uint32_t bad = 0;
     VBX_CUDA(c, cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
     VBX_CUDA(c, cudaStreamSynchronize(s));
     if (bad) return fail(c, VBX_E_INVALID, "debug_apply: a block is not in the TSDF layer");
-    Marks mk;
-    mk.c = c;
-    mk.s = s;
+    Marks mk{c, s, x.marks};
     uint64_t launches = 0;
     const GivenRecords given{d_sdf, d_w, d_col};
-    if (int rc = sort_and_apply(c, mk, &launches, &given)) return rc;
-    VBX_CUDA(c, cudaMemcpyAsync(c->h_state, c->d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+    if (int rc = sort_and_apply(c, x, mk, &launches, nullptr, &given)) return rc;
+    VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
     VBX_CUDA(c, cudaStreamSynchronize(s));
     VBX_CUDA(c, cudaGetLastError());
-    if (int rc = check_state_errors(c, c->h_state->error)) return rc;
-    for (int i = 0; i < 16; ++i) c->apply_paths[i] = i < kApplyPaths ? c->h_state->apply_paths[i] : 0;
+    if (int rc = check_state_errors(c, *S.h_state)) return rc;
+    for (int i = 0; i < 16; ++i) c->apply_paths[i] = i < kApplyPaths ? S.h_state->apply_paths[i] : 0;
     if (paths) std::memcpy(paths, c->apply_paths, sizeof(c->apply_paths));
     return VBX_OK;
   };
@@ -3148,16 +3155,18 @@ int debug_apply(vbx_ctx* c, const int32_t* idx3, uint32_t nb, uint64_t n, const 
 // exclusive prefix sum of n host uint32 through the engine's scan kernel
 int debug_scan(vbx_ctx* c, const uint32_t* in, uint32_t n, uint32_t* out) {
   cudaStream_t s = c->stream;
+  const vbx_ctx::ScratchSet& S = c->set[0];
+  uint32_t* status = c->lane[0].scan_status;
   if (n > c->max_points + 1) return fail(c, VBX_E_CAPACITY, "debug_scan: n > max_points_per_scan + 1");
-  VBX_CUDA(c, cudaMemcpyAsync(c->cnt, in, (size_t)n * 4, cudaMemcpyHostToDevice, s));
+  VBX_CUDA(c, cudaMemcpyAsync(S.cnt, in, (size_t)n * 4, cudaMemcpyHostToDevice, s));
   const uint32_t tiles = (n + kScanTile - 1) / kScanTile;
-  VBX_CUDA(c, cudaMemsetAsync(c->scan_status, 0, (size_t)(tiles + 1) * sizeof(uint32_t), s));
+  VBX_CUDA(c, cudaMemsetAsync(status, 0, (size_t)(tiles + 1) * sizeof(uint32_t), s));
   if (n) {
-    k_exclusive_scan<<<std::min<uint32_t>(tiles, c->grid_sms * 4), kSortThreads, 0, s>>>(c->cnt, nullptr, nullptr, c->off, nullptr, n,
-                                                                               c->scan_status + 1, c->scan_status, nullptr,
+    k_exclusive_scan<<<std::min<uint32_t>(tiles, c->grid_sms * 4), kSortThreads, 0, s>>>(S.cnt, nullptr, nullptr, S.off, nullptr, n,
+                                                                               status + 1, status, nullptr,
                                                                                nullptr, nullptr, 0ull, 0u);
   }
-  VBX_CUDA(c, cudaMemcpyAsync(out, c->off, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(out, S.off, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));
   VBX_CUDA(c, cudaGetLastError());
   return VBX_OK;
