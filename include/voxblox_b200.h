@@ -165,8 +165,11 @@ VBX_API int vbx_tsdf_integrate_device(vbx_ctx* ctx, int kind, const float q_wxyz
  * integrate calls since vbx_create   [9] / [10] bundles / points folded a second time with IEEE
  * division (diagnostic)   [11] passes the call needed (> 1 when its update records exceed
  * vbx_engine_options.max_updates_per_pass: the synchronous calls then emit and apply contiguous
- * ray ranges one after the other, same result; [3] counts a voxel once per pass)  [12..15] reserved
- * After asynchronous submissions: the counters of the last scan collected (all, after vbx_sync). */
+ * ray ranges one after the other, same result; [3] counts a voxel once per pass)  [12] bits a Merged
+ * bundle key uses   [13] asynchronously submitted scans redone synchronously since vbx_create
+ * [14] / [15] host time (ns) vbx_tsdf_integrate_async spent waiting for a free hand-off set / enqueueing,
+ * summed since vbx_create.
+ * After asynchronous submissions: [0..12] are those of the last scan collected (all, after vbx_sync). */
 VBX_API int vbx_get_counters(const vbx_ctx* ctx, uint64_t out[16]);
 /* Device time (ms, CUDA events on the context's stream) of the last integrate /
  * ESDF update call, excluding host<->device copies of the cloud. */
@@ -330,8 +333,8 @@ VBX_API int vbx_block_owner(const vbx_ctx* ctx, const int32_t block_index[3], in
  * stage boundaries and accumulates per-stage device time:
  *   TSDF  [0] point keys  [1] point sort  [2] ray count + block allocation  [3] scan
  *         [4] slot assign [5] ray emit    [6] update sort                   [7] apply
- *         [8] bundle heads + merge
- *   ESDF  [9] propagate   [10] raise      [11] lower wavefront              [12..15] reserved
+ *         [8] bundle merge        [12] bundle heads + order
+ *   ESDF  [9] propagate   [10] raise      [11] lower wavefront              [13..15] reserved
  * calls[i] counts how many times stage i ran. */
 /* Page-locked host buffers for point clouds: vbx_tsdf_integrate copies asynchronously (and at
  * full PCIe rate) only from memory that is page-locked; anything else is staged by the driver.

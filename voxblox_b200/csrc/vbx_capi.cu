@@ -66,19 +66,7 @@ void harvest_async(vbx_ctx* c, vbx_ctx::ScratchSet& S) {
   S.in_flight = false;
   const ScanState& h = *S.h_state;
   c->n_blocks = std::max(c->n_blocks, h.n_blocks);
-  std::memset(c->counters, 0, sizeof(c->counters));
-  c->counters[0] = h.n_rays;
-  c->counters[1] = h.n_clear_rays;
-  c->counters[2] = h.total_found;
-  if (h.total_found) c->record_hint = h.total_found;
-  if (S.kind == VBX_MERGED && !(h.error & kFatalErrors)) c->bundle_hint = std::max(h.n_rays, h.n_clear_rays);
-  c->counters[3] = h.n_voxels;
-  c->counters[4] = h.n_touched;
-  c->counters[5] = h.n_new;
-  c->counters[6] = S.kind == VBX_MERGED ? h.n_valid_points : (uint64_t)h.n_rays + h.n_clear_rays;
-  c->counters[7] = S.launches;
-  c->counters[11] = 1;
-  for (int i = 0; i < kApplyPaths; ++i) c->apply_paths[i] = h.apply_paths[i];
+  report_scan(c, h, S.kind, S.launches, 1, h.n_new);
   const uint32_t fatal = h.error & kFatalErrors & ~kErrUpdatesFull;
   if (!fatal && (h.error & (kErrUpdatesFull | kSkipped))) {
     // more update records than one pass holds (or queued behind such a scan): nothing was applied;
@@ -617,10 +605,10 @@ int vbx_debug_apply_paths(const vbx_ctx* c, uint64_t out[16]) {
 int vbx_get_counters(const vbx_ctx* c, uint64_t out[16]) {
   if (!c || !out) return VBX_E_INVALID;
   std::memcpy(out, c->counters, sizeof(c->counters));
-  out[8] = c->launches;  // kernels launched by TSDF integration since vbx_create
-  out[13] = c->async_redone;  // asynchronously submitted scans that were redone synchronously (see vbx_tsdf_integrate_async)
-  out[14] = c->async_wait_ns;    // host time asynchronous submissions spent waiting for a free hand-off set ...
-  out[15] = c->async_submit_ns;  // ... and enqueueing (cumulative, ns)
+  out[kCntLaunchesTotal] = c->launches;
+  out[kCntAsyncRedone] = c->async_redone;
+  out[kCntAsyncWaitNs] = c->async_wait_ns;
+  out[kCntAsyncSubmitNs] = c->async_submit_ns;
   return VBX_OK;
 }
 

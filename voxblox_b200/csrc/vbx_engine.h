@@ -348,13 +348,11 @@ struct vbx_ctx {
   float* icp_out_host = nullptr;
   uint64_t icp_cap = 0;
   // reporting
-  uint32_t last_passes = 1;  // passes the last synchronous integrate call needed (K > max_updates_per_pass)
   uint64_t counters[16] = {0};
   uint64_t apply_paths[16] = {0};  // ScanState::apply_paths of the last call whose status reached the host
   bool count_apply_paths = false;  // k_apply counts its paths (vbx_debug_count_apply_paths; vbx_debug_apply always does)
   uint64_t async_wait_ns = 0, async_submit_ns = 0;  // host time of vbx_tsdf_integrate_async: waiting for a hand-off set / enqueueing
   uint64_t esdf_counters[16] = {0};
-  uint64_t shard_front_counters[4] = {0};
   float last_ms = 0.f;
   uint64_t launches = 0;
   cudaEvent_t tev0 = nullptr, tev1 = nullptr;  // vbx_timer_*
@@ -402,6 +400,51 @@ struct ScanRoute {
 inline ScanRoute sync_route(vbx_ctx* c) { return {c->set[0], c->lane[0], c->stream, c->grid_sms, c->profiling}; }
 int integrate_device(vbx_ctx* c, const ScanRoute& x, int kind, const float q[4], const float t[3], const float* d_xyz,
                      const uint8_t* d_rgba, uint64_t n, int freespace);
+
+// The slots of vbx_get_stage_ms, in the order of api.py's STAGE_NAMES (the C-ABI's order)
+enum Stage : int {
+  kStagePointKeys, kStagePointSort, kStageRayCount, kStageScan, kStageAssign, kStageRayEmit, kStageUpdateSort,
+  kStageApply, kStageBundleMerge, kStageEsdfPropagate, kStageEsdfRaise, kStageEsdfLower, kStageBundleOrder
+};
+
+// One call's bookkeeping: the kernels it launched, counted where each is launched, and with stage profiling
+// on an event at the end of each stage on stream s (off while a graph is captured: stage events would
+// serialise the streams).
+struct Tally {
+  vbx_ctx* c;
+  cudaStream_t s;
+  bool on;
+  uint64_t launches = 0;
+  int n = 0;
+  Stage stage[19];
+  void begin() {
+    if (on) cudaEventRecord(c->sev[0], s);
+  }
+  void mark(Stage just_finished) {
+    if (on && n < 19) {
+      cudaEventRecord(c->sev[n + 1], s);
+      stage[n++] = just_finished;
+    }
+  }
+  void collect() {
+    for (int m = 0; m < n; ++m) {
+      float ms = 0.f;
+      if (cudaEventElapsedTime(&ms, c->sev[m], c->sev[m + 1]) == cudaSuccess) {
+        c->stage_ms[stage[m]] += ms;
+        c->stage_calls[stage[m]] += 1;
+      }
+    }
+  }
+};
+
+// The slots of vbx_get_counters (include/voxblox_b200.h)
+enum Counter : int {
+  kCntRays, kCntClearRays, kCntUpdates, kCntVoxels, kCntBlocksTouched, kCntBlocksAllocated, kCntValidPoints,
+  kCntLaunches, kCntLaunchesTotal, kCntRefoldedBundles, kCntRefoldedPoints, kCntPasses, kCntBundleKeyBits,
+  kCntAsyncRedone, kCntAsyncWaitNs, kCntAsyncSubmitNs
+};
+// A finished TSDF call's status block -> its counters, the grid hints of later scans and the apply-path counts
+void report_scan(vbx_ctx* c, const ScanState& h, int kind, uint64_t launches, uint64_t passes, uint64_t blocks_allocated);
 }  // namespace vbx
 
 #define VBX_CUDA(c, expr)                                          \

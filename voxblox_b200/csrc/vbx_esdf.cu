@@ -827,7 +827,7 @@ int esdf_add_robot_position(vbx_ctx* c, const float p[3]) {
   cudaStream_t s = c->stream;
   const vbx_esdf_config& cfg = c->ecfg;
   std::memset(c->esdf_counters, 0, sizeof(c->esdf_counters));
-  uint64_t launches = 0;
+  Tally tally{c, s, false};
   const float radii[2] = {cfg.clear_sphere_radius, cfg.occupied_sphere_radius};
   SphereParams S[2];
   std::vector<float> xs[2];
@@ -853,20 +853,21 @@ int esdf_add_robot_position(vbx_ctx* c, const float p[3]) {
   VBX_CUDA(c, cudaEventRecord(c->ev0, s));
   VBX_CUDA(c, cudaMemsetAsync(d_state, 0, sizeof(ScanState), s));
   k_esdf_set_pending<<<1, 1, 0, s>>>(d_state, c->esdf_pending_raise, c->esdf_pending_open);
+  ++tally.launches;
   for (int k = 0; k < 2; ++k) {
     if (S[k].n == 0) continue;
     VBX_CUDA(c, cudaMemcpyAsync(d_xs[k], xs[k].data(), xs[k].size() * sizeof(float), cudaMemcpyHostToDevice, s));
     const uint64_t n3 = (uint64_t)S[k].n * S[k].n * S[k].n;
     k_esdf_sphere_blocks<<<grid_for(n3, 256), 256, 0, s>>>(S[k], c->tab, d_xs[k], d_state);
-    launches += 1;
+    ++tally.launches;
   }
   k_esdf_sphere_assign<<<grid_for(c->tab.max_blocks, 256), 256, 0, s>>>(c->tab, c->n_blocks, d_state);
-  launches += 2;
+  ++tally.launches;
   for (int k = 0; k < 2; ++k) {
     if (S[k].n == 0) continue;
     const uint64_t n3 = (uint64_t)S[k].n * S[k].n * S[k].n;
     k_esdf_sphere_apply<<<grid_for(n3, 256), 256, 0, s>>>(S[k], c->tab, d_xs[k], c->raise_q[0], c->frontier[0], d_state);
-    launches += 1;
+    ++tally.launches;
   }
   VBX_CUDA(c, cudaEventRecord(c->ev1, s));
   VBX_CUDA(c, cudaMemcpyAsync(c->set[0].h_state, d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
@@ -886,8 +887,8 @@ int esdf_add_robot_position(vbx_ctx* c, const float p[3]) {
   c->esdf_counters[2] = h.esdf_counts[2]; // voxels set occupied
   c->esdf_counters[4] = h.raise_n[0];     // queued: raise_
   c->esdf_counters[5] = h.frontier_n[0];  // queued: open_
-  c->esdf_counters[7] = launches;
-  c->launches += launches;
+  c->esdf_counters[7] = tally.launches;
+  c->launches += tally.launches;
   return refresh_host_mirror(c);
 }
 
@@ -940,7 +941,7 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
   E.d2 = E.u2 * c->voxel_size;
   E.d3 = E.u3 * c->voxel_size;
   E.cap = (uint32_t)c->frontier_cap;
-  uint64_t launches = 0;
+  Tally tally{c, s, c->profiling};
   if (E.full_euclidean && !c->esdf_fe) {
     VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_fe),
                            (size_t)c->tab.max_blocks * c->vox_per_block * sizeof(unsigned long long)));
@@ -948,7 +949,7 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
   ScanState* d_state = c->set[0].d_state;  // hand-off set 0's status block
   const ScanState& h = *c->set[0].h_state;
   VBX_CUDA(c, cudaEventRecord(c->ev0, s));
-  if (c->profiling) cudaEventRecord(c->sev[0], s);
+  tally.begin();
   VBX_CUDA(c, cudaMemsetAsync(d_state, 0, sizeof(ScanState), s));
   if (c->n_blocks == 0) {
     VBX_CUDA(c, cudaStreamSynchronize(s));
@@ -964,7 +965,7 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
   const bool pending = c->esdf_pending_raise || c->esdf_pending_open;
   if (pending) {
     k_esdf_set_pending<<<1, 1, 0, s>>>(d_state, c->esdf_pending_raise, c->esdf_pending_open);
-    launches += 1;
+    ++tally.launches;
   }
   c->esdf_pending_raise = c->esdf_pending_open = 0;
   if (batch) {
@@ -981,6 +982,7 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
       VBX_CUDA(c, cudaMemcpyAsync(c->esdf_block_list, listed_slots, (size_t)nb * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
       VBX_CUDA(c, cudaMemcpyAsync(&d_state->esdf_counts[0], &nb, sizeof(uint32_t), cudaMemcpyHostToDevice, s));
       k_esdf_mark_listed<<<grid_for(nb, 256), 256, 0, s>>>(c->tab, c->esdf_block_list, nb);
+      ++tally.launches;
       VBX_CUDA(c, cudaStreamSynchronize(s));  // the two host sources above are stack / vector memory
     }
   } else {
@@ -988,24 +990,25 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
     // the call; the launches below are sized for the upper bound (every slot) and the kernels stop at
     // the real count
     k_esdf_block_list<<<grid_for(c->n_blocks, 256), 256, 0, s>>>(c->tab, c->n_blocks, batch, c->esdf_block_list, d_state);
+    ++tally.launches;
     nb = c->n_blocks;
   }
-  launches += 1;
   if (nb > 0 || pending) {
     if (nb > 0) {
       // one thread block per voxel block, both slabs staged by the TMA
       const size_t slab_bytes = (size_t)c->vox_per_block * (sizeof(TsdfVoxel) + sizeof(EsdfVoxel));
       k_esdf_propagate<<<nb, (unsigned int)std::max<uint32_t>(32u, std::min<uint32_t>(1024u, c->vox_per_block)), slab_bytes, s>>>(
           E, c->tab, c->esdf_block_list, nb, c->frontier[0], c->raise_q[0], c->esdf_seed_list, d_state);
-      launches += 1;
+      ++tally.launches;
     }
     if (nb > 0 && incremental) {
       const unsigned int g = c->grid_sms * 8;
       k_esdf_seed<<<g, 256, 0, s>>>(E, c->tab, c->esdf_seed_list, c->frontier[0], c->esdf_seed_val, d_state);
+      ++tally.launches;
       k_esdf_seed_commit<<<g, 256, 0, s>>>(E, c->tab, c->esdf_seed_list, c->esdf_seed_val, d_state);
-      launches += 2;
+      ++tally.launches;
     }
-    if (c->profiling) cudaEventRecord(c->sev[1], s);
+    tally.mark(kStageEsdfPropagate);
     {
       int per_sm = (nb <= 256 && !pending) ? c->esdf_ctas_small : c->esdf_ctas_wide;
       if (const char* e = std::getenv("VBX_ESDF_CTAS")) per_sm = std::max(1, std::min(std::atoi(e), c->esdf_ctas_wide));  // (tuning aid)
@@ -1014,24 +1017,26 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
     {
       void* args[] = {&E, &c->tab, &c->raise_q[0], &c->raise_q[1], &c->frontier[0], &d_state};
       VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_esdf_raise, dim3(c->esdf_grid_raise), dim3(256), args, 0, s));
+      ++tally.launches;
     }
-    if (c->profiling) cudaEventRecord(c->sev[2], s);
+    tally.mark(kStageEsdfRaise);
     long long* fe = nullptr;
     if (E.full_euclidean) {
       fe = reinterpret_cast<long long*>(c->esdf_fe);
       k_esdf_fe_pack<<<c->grid_sms * 8, 256, 0, s>>>(c->tab, (uint64_t)c->n_blocks * c->vox_per_block, fe, d_state);
-      launches += 1;
+      ++tally.launches;
     }
     {
       void* args[] = {&E, &c->tab, &c->frontier[0], &c->frontier[1], &c->esdf_touched, &fe, &d_state};
       VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_esdf_lower, dim3(c->esdf_grid_lower), dim3(256), args, 0, s));
+      ++tally.launches;
     }
     k_esdf_parents<<<c->grid_sms * 8, 256, 0, s>>>(E, c->tab, c->esdf_touched, fe, d_state);
-    if (c->profiling) cudaEventRecord(c->sev[3], s);
-    launches += 3;
+    ++tally.launches;
+    tally.mark(kStageEsdfLower);
     if (nb > 0 && !batch && clear_updated_flag) {
       k_esdf_clear_tsdf_flag<<<grid_for(nb, 256), 256, 0, s>>>(c->tab, c->esdf_block_list, d_state);
-      launches += 1;
+      ++tally.launches;
     }
   }
   VBX_CUDA(c, cudaEventRecord(c->ev1, s));
@@ -1039,22 +1044,14 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
   VBX_CUDA(c, cudaStreamSynchronize(s));
   VBX_CUDA(c, cudaGetLastError());
   VBX_CUDA(c, cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
-  if (c->profiling && (nb > 0 || pending)) {
-    for (int m = 0; m < 3; ++m) {
-      float ms = 0.f;
-      if (cudaEventElapsedTime(&ms, c->sev[m], c->sev[m + 1]) == cudaSuccess) {
-        c->stage_ms[9 + m] += ms;
-        c->stage_calls[9 + m] += 1;
-      }
-    }
-  }
+  tally.collect();
   if (h.error & kErrUpdatesFull) return fail(c, VBX_E_CAPACITY, "ESDF wavefront queue capacity exceeded");
   if (h.error & kErrParentRange) {
     return fail(c, VBX_E_CAPACITY, "full-Euclidean ESDF: a parent vector component left [-512, 511] voxels");
   }
   for (int i = 0; i < 7; ++i) c->esdf_counters[i] = h.esdf_counts[i];
-  c->esdf_counters[7] = launches;
-  c->launches += launches;
+  c->esdf_counters[7] = tally.launches;
+  c->launches += tally.launches;
   return VBX_OK;
 }
 

@@ -237,9 +237,8 @@ k_point_bounds(const ScanArgs* __restrict__ A, uint32_t* __restrict__ first_bits
 
 // Merged, pass 2: key every point by its end voxel (bundleRays, cc:340-371), in the reference's
 // point order (position s of that order holds point point_order(s)).
-template <typename KeyT>
 __global__ void k_point_keys(const ScanArgs* __restrict__ A, const uint32_t* __restrict__ order,
-                             KeyT* __restrict__ keys, uint32_t* __restrict__ vals, ScanState* st) {
+                             uint64_t* __restrict__ keys, uint32_t* __restrict__ vals, ScanState* st) {
   const ScanParams P = A->P;
   const float* __restrict__ xyz = A->xyz;
   const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
@@ -249,12 +248,12 @@ __global__ void k_point_keys(const ScanArgs* __restrict__ A, const uint32_t* __r
     const uint32_t idx = point_order(P, order, s);
     const F3 p = load_point(xyz, idx);
     const int cls = classify_point(p, P.min_ray, P.max_ray, P.allow_clear != 0, P.freespace != 0);
-    KeyT key = (KeyT)~(KeyT)0;
+    uint64_t key = kInvalidPointKey;
     if (cls != 0) {
       const I3 v = grid_index(transform(P.T, p), P.voxel_size_inv);
       bool in_range;
       const uint64_t k = make_point_key(kl, v, cls == 2, &in_range);
-      if (in_range) key = (KeyT)k;  // (out of range only beyond +-2^20 voxels: flagged by k_point_bounds)
+      if (in_range) key = k;  // (out of range only beyond +-2^20 voxels: flagged by k_point_bounds)
     }
     keys[s] = key;
     vals[s] = idx;
@@ -294,8 +293,7 @@ constexpr uint32_t kHeadBig = 0x80000000u;   // head_list entry: sorted position
 // first of its bundle, i.e. the point whose operator[] inserts the bundle's key into the reference's
 // voxel_map / clear_map (bundleRays, cc:340-371).  k_bundle_order turns them into the maps'
 // iteration order.
-template <typename KeyT>
-__global__ void k_heads(const ScanArgs* __restrict__ A, const KeyT* __restrict__ keys, const uint32_t* __restrict__ vals,
+__global__ void k_heads(const ScanArgs* __restrict__ A, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals,
                         const uint32_t* __restrict__ order_inv, uint32_t* __restrict__ head_list,
                         uint32_t* __restrict__ big_list, uint32_t* __restrict__ first_bits, uint32_t* __restrict__ cnt,
                         ScanState* st) {
@@ -306,8 +304,8 @@ __global__ void k_heads(const ScanArgs* __restrict__ A, const KeyT* __restrict__
   bool head = false;
   if (i <= n) cnt[i] = 0;
   if (i < n) {
-    const KeyT key = keys[i];
-    head = key != (KeyT)~(KeyT)0 && (i == 0 || keys[i - 1] != key);
+    const uint64_t key = keys[i];
+    head = key != kInvalidPointKey && (i == 0 || keys[i - 1] != key);
     if (head) {
       // the stable sort keeps point order inside a bundle: its first member is its first occurrence
       const uint32_t t0 = point_order_inv(P, order_inv, vals[i]);
@@ -374,8 +372,7 @@ k_order_prefix(const ScanArgs* __restrict__ A, const uint32_t* __restrict__ firs
   }
 }
 
-template <typename KeyT>
-__global__ void k_order_heads(const ScanArgs* __restrict__ A, const KeyT* __restrict__ keys, const uint32_t* __restrict__ vals,
+__global__ void k_order_heads(const ScanArgs* __restrict__ A, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals,
                               const uint32_t* __restrict__ order_inv, const uint32_t* __restrict__ head_list,
                               const uint32_t* __restrict__ first_bits, OrderScratch g, const ScanState* st) {
   const ScanParams P = A->P;
@@ -639,12 +636,12 @@ __device__ __forceinline__ float fold_step_colour(float state, float4 abcd) {
 //   merged = (merged * W + p * w) / (W + w); colour blended; W += w            (cc:387-405)
 // Lanes 0-2 carry x, y, z of the mean, lanes 3-6 the colour channels (floats holding exact
 // integers 0..255).  Returns true if the fast division met an operand it does not trust.
-template <typename KeyT, bool kIeee>
+template <bool kIeee>
 __device__ bool fold_bundle(const ScanParams& P, const float* __restrict__ xyz, const uint8_t* __restrict__ rgba,
-                            const KeyT* __restrict__ keys, const uint32_t* __restrict__ vals, uint32_t i,
+                            const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals, uint32_t i,
                             float4* stage_warp, F3* out_mp, float* out_mw, uint32_t* out_col, const ScanState* st) {
   const int lane = threadIdx.x & 31;
-  const KeyT key = keys[i];
+  const uint64_t key = keys[i];
   const bool clearing = key_is_clearing(key_layout(st), (uint64_t)key);
   float mw = 0.0f;
   bool done = false;
@@ -659,18 +656,18 @@ __device__ bool fold_bundle(const ScanParams& P, const float* __restrict__ xyz, 
   // Three-deep load pipeline: while chunk c is folded, the points of chunk c+1 are gathered (their
   // keys / point indices arrived one iteration ago) and the keys / indices of chunk c+2 are
   // requested -- no load is waited for right after it was issued.
-  KeyT k_next;
+  uint64_t k_next;
   uint32_t idx_next;
   bool inb_next;
   {
     const uint32_t jj = j0 + lane;
     const bool inb = jj < P.n;
-    const KeyT kk = inb ? keys[jj] : (KeyT)~(KeyT)0;
+    const uint64_t kk = inb ? keys[jj] : kInvalidPointKey;
     const uint32_t idx = inb ? vals[jj] : 0u;
     j0 += 32;
     const uint32_t jn = j0 + lane;
     inb_next = jn < P.n;
-    k_next = inb_next ? keys[jn] : (KeyT)~(KeyT)0;
+    k_next = inb_next ? keys[jn] : kInvalidPointKey;
     idx_next = inb_next ? vals[jn] : 0u;
     in = inb && kk == key;
     if (in) {
@@ -692,7 +689,7 @@ __device__ bool fold_bundle(const ScanParams& P, const float* __restrict__ xyz, 
       j0 += 32;
       const uint32_t jn = j0 + lane;
       inb_next = jn < P.n;
-      k_next = inb_next ? keys[jn] : (KeyT)~(KeyT)0;
+      k_next = inb_next ? keys[jn] : kInvalidPointKey;
       idx_next = inb_next ? vals[jn] : 0u;
     }
     const float w = inc ? point_weight(pc.z, P.use_const_weight != 0) : 0.f;
@@ -817,10 +814,9 @@ __device__ __forceinline__ void consumer_barrier(int triple_in_block) {
 // so the preparation of chunk c+1 overlaps the chains of chunk c (two shared-memory slots, one
 // named barrier per chunk), also across bundle boundaries, and each chain issues only its own
 // instructions (~5 dependent operations per member for the mean, ~7 for a colour channel).
-template <typename KeyT>
 __global__ void __launch_bounds__(192)
 k_merge(const ScanArgs* __restrict__ A,
-        const KeyT* __restrict__ keys, const uint32_t* __restrict__ vals, const uint32_t* __restrict__ head_list,
+        const uint64_t* __restrict__ keys, const uint32_t* __restrict__ vals, const uint32_t* __restrict__ head_list,
         const uint32_t* __restrict__ big_list,
         float4* __restrict__ ray_p, float4* __restrict__ ray_a, uint2* __restrict__ ray_c, uint32_t* __restrict__ cnt,
         ScanState* st) {
@@ -858,7 +854,7 @@ k_merge(const ScanArgs* __restrict__ A,
         if (hl & kHeadBig) continue;  // folded through the big list
       }
       const uint32_t i = hl & ~kHeadBig;
-      const KeyT key = keys[i];
+      const uint64_t key = keys[i];
       const bool clearing = key_is_clearing(kl, (uint64_t)key);
       float mw = 0.0f;
       bool done = false, first = true;
@@ -868,18 +864,18 @@ k_merge(const ScanArgs* __restrict__ A,
       uint32_t col = 0u;
       // three-deep load pipeline: while chunk c is prepared, the points of chunk c+1 are gathered
       // (their keys / point indices arrived one iteration ago) and the keys of chunk c+2 requested
-      KeyT k_next;
+      uint64_t k_next;
       uint32_t idx_next;
       bool inb_next;
       {
         const uint32_t jj = j0 + lane;
         const bool inb = jj < P.n;
-        const KeyT kk = inb ? keys[jj] : (KeyT)~(KeyT)0;
+        const uint64_t kk = inb ? keys[jj] : kInvalidPointKey;
         const uint32_t idx = inb ? vals[jj] : 0u;
         j0 += 32;
         const uint32_t jn = j0 + lane;
         inb_next = jn < P.n;
-        k_next = inb_next ? keys[jn] : (KeyT)~(KeyT)0;
+        k_next = inb_next ? keys[jn] : kInvalidPointKey;
         idx_next = inb_next ? vals[jn] : 0u;
         in = inb && kk == key;
         if (in) {
@@ -901,7 +897,7 @@ k_merge(const ScanArgs* __restrict__ A,
           j0 += 32;
           const uint32_t jn = j0 + lane;
           inb_next = jn < P.n;
-          k_next = inb_next ? keys[jn] : (KeyT)~(KeyT)0;
+          k_next = inb_next ? keys[jn] : kInvalidPointKey;
           idx_next = inb_next ? vals[jn] : 0u;
         }
         const float w = inc ? point_weight(pc.z, P.use_const_weight != 0) : 0.f;
@@ -1052,11 +1048,11 @@ k_merge(const ScanArgs* __restrict__ A,
         if (__any_sync(0xffffffffu, suspect)) {
           // the fast division met an operand it does not trust: fold this bundle again with the
           // IEEE division (this warp alone, the slot just consumed as its staging area)
-          fold_bundle<KeyT, true>(P, xyz, rgba, keys, vals, i, stage[pair_in_block][slot], &mp, &mw, &mcol, st);
+          fold_bundle<true>(P, xyz, rgba, keys, vals, i, stage[pair_in_block][slot], &mp, &mw, &mcol, st);
           if (lane == 0) {
             atomicAdd(&st->n_refold, 1u);
             uint32_t lo = i, hi = P.n;  // first sorted position with a larger key
-            const KeyT k = keys[i];
+            const uint64_t k = keys[i];
             while (lo < hi) {
               const uint32_t mid = (lo + hi) >> 1;
               if (keys[mid] <= k) lo = mid + 1; else hi = mid;
@@ -1084,8 +1080,7 @@ k_merge(const ScanArgs* __restrict__ A,
 
 // binary search over the sorted point keys: is there a NORMAL bundle ending in this voxel?
 // (the voxel_map.find() of the anti-grazing test, cc:415-422)
-template <typename KeyT>
-__device__ bool bundle_exists(const KeyT* keys, uint32_t n, KeyT key) {
+__device__ bool bundle_exists(const uint64_t* keys, uint32_t n, uint64_t key) {
   uint32_t lo = 0, hi = n;
   while (lo < hi) {
     const uint32_t mid = (lo + hi) >> 1;
@@ -1098,14 +1093,13 @@ __device__ bool bundle_exists(const KeyT* keys, uint32_t n, KeyT key) {
   return lo < n && keys[lo] == key;
 }
 
-template <typename KeyT>
-__device__ __forceinline__ bool grazing_skip(const ScanParams& P, const KeyLayout& kl, const KeyT* keys, KeyT own,
+__device__ __forceinline__ bool grazing_skip(const ScanParams& P, const KeyLayout& kl, const uint64_t* keys, uint64_t own,
                                              bool clearing, int x, int y, int z) {
   bool in_range;
-  const KeyT vkey = (KeyT)normal_key_of(kl, x, y, z, &in_range);
+  const uint64_t vkey = normal_key_of(kl, x, y, z, &in_range);
   if (!in_range) return false;
-  const KeyT own_normal = clearing ? (KeyT)~(KeyT)0 : own;
-  return (clearing || vkey != own_normal) && bundle_exists<KeyT>(keys, P.n, vkey);
+  const uint64_t own_normal = clearing ? kInvalidPointKey : own;
+  return (clearing || vkey != own_normal) && bundle_exists(keys, P.n, vkey);
 }
 
 // ApproxHashSet::replaceHash, utils/approx_hash_array.h:125-134.  The generation tag in
@@ -1119,9 +1113,8 @@ __device__ __forceinline__ bool replace_hash(unsigned long long* set, uint32_t h
 // One thread per ray: first DDA walk.  Merged rays come from k_merge's records through the
 // dense ray list; Simple / Fast build their ray from point slot i (integrateFunction,
 // cc:269-305 / :488-553).
-template <typename KeyT>
 __global__ void k_rays_count(const ScanArgs* __restrict__ A, Tables tab, const uint32_t* __restrict__ order,
-                             const KeyT* __restrict__ keys, const uint32_t* __restrict__ head_list,
+                             const uint64_t* __restrict__ keys, const uint32_t* __restrict__ head_list,
                              float4* __restrict__ ray_p, float4* __restrict__ ray_a, uint2* __restrict__ ray_c,
                              uint32_t* __restrict__ cnt,
                              unsigned long long* set_start, unsigned long long* set_observed, ScanState* st) {
@@ -1132,7 +1125,7 @@ __global__ void k_rays_count(const ScanArgs* __restrict__ A, Tables tab, const u
   uint32_t i;
   F3 point_G;
   bool clearing;
-  KeyT own = 0;
+  uint64_t own = 0;
   if (P.kind == VBX_MERGED) {
     if (t >= st->n_ray_list) return;
     i = t;  // bundle id j (the count does not depend on the order); head_list[j] = sorted position of its head
@@ -1182,7 +1175,7 @@ __global__ void k_rays_count(const ScanArgs* __restrict__ A, Tables tab, const u
   const int lim = (kCoordBias - 1) << P.L;
   for (unsigned int s = 0; s <= d.len; ++s, dda_advance(d)) {
     if (P.kind == VBX_MERGED && P.anti_grazing) {
-      if (grazing_skip<KeyT>(P, key_layout(st), keys, own, clearing, d.cx, d.cy, d.cz)) continue;
+      if (grazing_skip(P, key_layout(st), keys, own, clearing, d.cx, d.cy, d.cz)) continue;
     }
     if (P.kind == VBX_FAST) {
       // cc:531-543: stop once the ray runs through voxels other rays already observed
@@ -1372,8 +1365,8 @@ struct ScanBlockIds {
 
 // One ray, walked sequentially by the calling thread: RayCaster's loop (integrator_utils.cc:106-125)
 // with allocateStorageAndGetVoxelPtr's find-or-create per block change (cc:91-134), through block_id.
-template <typename KeyT, typename BlockIds>
-__device__ void emit_ray_sequential(const ScanParams& P, const BlockIds& block_id, const KeyT* __restrict__ keys,
+template <typename BlockIds>
+__device__ void emit_ray_sequential(const ScanParams& P, const BlockIds& block_id, const uint64_t* __restrict__ keys,
                                     uint32_t i, uint32_t rank, uint32_t head_pos, const float4* __restrict__ ray_p,
                                     const uint32_t* __restrict__ cnt,
                                     const uint32_t* __restrict__ off, uint32_t* __restrict__ ckeys,
@@ -1387,7 +1380,7 @@ __device__ void emit_ray_sequential(const ScanParams& P, const BlockIds& block_i
   Dda d;
   dda_setup(d, P.origin, point_G, clearing, P.carving != 0, P.max_ray, P.voxel_size_inv, P.trunc,
             P.kind != VBX_FAST);
-  const KeyT own = (P.kind == VBX_MERGED) ? keys[head_pos] : (KeyT)0;
+  const uint64_t own = (P.kind == VBX_MERGED) ? keys[head_pos] : 0;
   uint32_t emitted = 0;
   int lbx = INT_MIN, lby = INT_MIN, lbz = INT_MIN;
   uint32_t tid = 0;
@@ -1396,7 +1389,7 @@ __device__ void emit_ray_sequential(const ScanParams& P, const BlockIds& block_i
   const int lim = (kCoordBias - 1) << P.L;
   for (unsigned int s = 0; s <= d.len && emitted < c; ++s, dda_advance(d)) {
     if (P.kind == VBX_MERGED && P.anti_grazing) {
-      if (grazing_skip<KeyT>(P, key_layout(st), keys, own, clearing, d.cx, d.cy, d.cz)) continue;
+      if (grazing_skip(P, key_layout(st), keys, own, clearing, d.cx, d.cy, d.cz)) continue;
     }
     const int bx = d.cx >> P.L, by = d.cy >> P.L, bz = d.cz >> P.L;
     if (bx != lbx || by != lby || bz != lbz) {
@@ -1421,8 +1414,7 @@ __device__ void emit_ray_sequential(const ScanParams& P, const BlockIds& block_i
   }
 }
 
-template <typename KeyT>
-__global__ void k_rays_emit(const ScanArgs* __restrict__ A, Tables tab, const KeyT* __restrict__ keys,
+__global__ void k_rays_emit(const ScanArgs* __restrict__ A, Tables tab, const uint64_t* __restrict__ keys,
                             const uint32_t* __restrict__ ray_list, const uint32_t* __restrict__ head_list,
                             const float4* __restrict__ ray_p, const uint32_t* __restrict__ cnt,
                             const uint32_t* __restrict__ off, uint32_t* __restrict__ ckeys,
@@ -1439,7 +1431,7 @@ __global__ void k_rays_emit(const ScanArgs* __restrict__ A, Tables tab, const Ke
     i = t;
     if (i >= P.n) return;
   }
-  emit_ray_sequential<KeyT>(P, HashBlockIds{P, tab, st}, keys, i, t, head_pos, ray_p, cnt, off, ckeys, cvals, st);
+  emit_ray_sequential(P, HashBlockIds{P, tab, st}, keys, i, t, head_pos, ray_p, cnt, off, ckeys, cvals, st);
 }
 
 // The same walk cast by a WARP per ray: the trace of the Merged integrator's single walk (a few
@@ -1461,9 +1453,8 @@ __global__ void k_rays_emit(const ScanArgs* __restrict__ A, Tables tab, const Ke
 constexpr int kChainCap = 256;
 constexpr int kWalkCap = 3 * kChainCap;
 
-template <typename KeyT>
 __global__ void __launch_bounds__(128)
-k_rays_emit_warp(const ScanArgs* __restrict__ A, ScanBlocks sb, const KeyT* __restrict__ keys, const uint32_t* __restrict__ ray_list,
+k_rays_emit_warp(const ScanArgs* __restrict__ A, ScanBlocks sb, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ ray_list,
                  const uint32_t* __restrict__ head_list, const float4* __restrict__ ray_p, const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ off,
                  uint32_t* __restrict__ ckeys, uint32_t* __restrict__ cvals, ScanState* st) {
   const ScanParams P = A->P;
@@ -1531,7 +1522,7 @@ k_rays_emit_warp(const ScanArgs* __restrict__ A, ScanBlocks sb, const KeyT* __re
     }
     if (!merge_ok) {
       if (lane == 0) {
-        emit_ray_sequential<KeyT>(P, block_id, keys, i, b, head_list[i] & ~kHeadBig, ray_p, cnt, off, ckeys, cvals, st);
+        emit_ray_sequential(P, block_id, keys, i, b, head_list[i] & ~kHeadBig, ray_p, cnt, off, ckeys, cvals, st);
       }
       __syncwarp();
       continue;
@@ -2155,32 +2146,6 @@ static int check_state_errors(vbx_ctx* c, const ScanState& h) {
 }
 
 namespace {
-struct Marks {
-  vbx_ctx* c;
-  cudaStream_t s;
-  bool on;  // (off while a graph is captured: stage events would serialise the streams)
-  int n = 0;
-  int stage[20];
-  void begin() {
-    if (on) cudaEventRecord(c->sev[0], s);
-  }
-  void mark(int stage_just_finished) {
-    if (on && n < 19) {
-      cudaEventRecord(c->sev[n + 1], s);
-      stage[n++] = stage_just_finished;
-    }
-  }
-  void collect() {
-    for (int m = 0; m < n; ++m) {
-      float ms = 0.f;
-      if (cudaEventElapsedTime(&ms, c->sev[m], c->sev[m + 1]) == cudaSuccess) {
-        c->stage_ms[stage[m]] += ms;
-        c->stage_calls[stage[m]] += 1;
-      }
-    }
-  }
-};
-
 // The back half's streams and hand-off events while a pipelined scan's graph is captured (capture_scan)
 struct Capture {
   cudaStream_t sort, apply;
@@ -2209,7 +2174,7 @@ static unsigned int sort_grid(const vbx_ctx* c, int which, uint64_t n_hint, unsi
 template <typename KeyT>
 static int own_sort(vbx_ctx* c, const ScanRoute& x, int which, KeyT* keys_a, uint32_t* vals_a, KeyT* keys_b,
                     uint32_t* vals_b, const unsigned long long* d_n, uint32_t n_fixed, uint64_t n_hint, int key_bits,
-                    bool result_in_a, uint64_t* launches, const uint32_t* d_key_bits = nullptr, bool plan_cleared = false) {
+                    bool result_in_a, Tally& tally, const uint32_t* d_key_bits = nullptr, bool plan_cleared = false) {
   cudaStream_t s = x.s;
   const int passes = std::min(kMaxPasses, (key_bits + 7) / 8);
   SortPlan* plan = which ? x.S.sort_plan1 : x.F.sort_plan0;
@@ -2219,7 +2184,7 @@ static int own_sort(vbx_ctx* c, const ScanRoute& x, int which, KeyT* keys_a, uin
   const unsigned int grid = sort_grid(c, which, n_hint, x.sms);
   k_sort<KeyT><<<grid, kSortThreads, 0, s>>>(keys_a, vals_a, keys_b, vals_b, d_n, n_fixed, passes, d_key_bits, plan, status,
                                               tiles_cap, result_in_a ? 1 : 0);
-  *launches += 1;
+  ++tally.launches;
   return VBX_OK;
 }
 
@@ -2250,14 +2215,14 @@ static OrderLaunch order_launch(const vbx_ctx* c, uint32_t n) {
   return o;
 }
 
-template <typename KeyT>
-static int launch_bundle_order(vbx_ctx* c, const ScanRoute& x, cudaStream_t so, uint32_t n, const KeyT* keys,
-                               const uint32_t* vals) {
+static int launch_bundle_order(vbx_ctx* c, const ScanRoute& x, cudaStream_t so, uint32_t n, Tally& tally) {
   const vbx_ctx::ScratchSet& S = x.S;
   const vbx_ctx::FrontLane& F = x.F;
   k_order_prefix<<<1, kOrderThreads, 0, so>>>(S.d_args, F.first_bits, F.order_scratch, S.d_state);
-  k_order_heads<KeyT><<<std::min<unsigned int>(grid_for(c->max_points, 256), x.sms * 2), 256, 0, so>>>(
-      S.d_args, keys, vals, c->order_inv, S.head_list, F.first_bits, F.order_scratch, S.d_state);
+  ++tally.launches;
+  k_order_heads<<<std::min<unsigned int>(grid_for(c->max_points, 256), x.sms * 2), 256, 0, so>>>(
+      S.d_args, S.pkeys0, F.pvals[0], c->order_inv, S.head_list, F.first_bits, F.order_scratch, S.d_state);
+  ++tally.launches;
   // Always a cooperative launch (the one-block form is a cooperative grid of one block), so that a scan
   // graph's node switches between the two forms by its grid and shared memory alone (update_scan_graph).
   const OrderLaunch o = order_launch(c, n);
@@ -2274,6 +2239,7 @@ static int launch_bundle_order(vbx_ctx* c, const ScanRoute& x, cudaStream_t so, 
   lc.numAttrs = 1;
   VBX_CUDA(c, cudaLaunchKernelEx(&lc, k_bundle_order, c->rehash, F.order_scratch, smem_words, S.ray_list,
                                  F.order_scratch.cta_tot, S.d_state));
+  ++tally.launches;
   return VBX_OK;
 }
 
@@ -2281,12 +2247,12 @@ static int launch_bundle_order(vbx_ctx* c, const ScanRoute& x, cudaStream_t so, 
 // private block table); every other walk creates blocks itself and runs in the back half.
 static bool traced_in_front(const ScanParams& P) { return P.kind == VBX_MERGED && P.single_walk; }
 
-template <typename KeyT>
-static void launch_trace(const ScanRoute& x, const KeyT* keys) {
+static void launch_trace(const ScanRoute& x, Tally& tally) {
   // a few thousand bundles of 100-300 steps: one warp per ray
   const vbx_ctx::ScratchSet& S = x.S;
-  k_rays_emit_warp<KeyT><<<x.sms * 8, 128, 0, x.s>>>(S.d_args, S.blocks, keys, S.ray_list, S.head_list, S.ray_p, S.cnt,
-                                                     S.off, S.ckeys[0], S.cvals[0], S.d_state);
+  k_rays_emit_warp<<<x.sms * 8, 128, 0, x.s>>>(S.d_args, S.blocks, S.pkeys0, S.ray_list, S.head_list, S.ray_p, S.cnt,
+                                               S.off, S.ckeys[0], S.cvals[0], S.d_state);
+  ++tally.launches;
 }
 
 // Stages up to the record offsets (for the Merged single walk also the trace that writes the update records):
@@ -2294,9 +2260,7 @@ static void launch_trace(const ScanRoute& x, const KeyT* keys) {
 // come from the set's argument block (S.d_args), and the grids are sized for max_points_per_scan -- surplus threads
 // exit at once -- so that one captured graph serves scans of any size (the point sort's grid, whose surplus
 // blocks would wait between passes, is set per scan instead: update_scan_graph).
-template <typename KeyT>
-static int front_half(vbx_ctx* c, const ScanRoute& x, const ScanParams& P, const uint32_t* order, Marks& mk,
-                      uint64_t* launches, const KeyT** keys_out) {
+static int front_half(vbx_ctx* c, const ScanRoute& x, const ScanParams& P, const uint32_t* order, Tally& tally) {
   cudaStream_t s = x.s;
   const vbx_ctx::ScratchSet& S = x.S;
   const vbx_ctx::FrontLane& F = x.F;
@@ -2305,61 +2269,58 @@ static int front_half(vbx_ctx* c, const ScanRoute& x, const ScanParams& P, const
   const uint32_t n = P.n;
   const uint32_t gn = c->max_points;
   const int TB = 256;
-  const KeyT* keys = nullptr;
-  const uint32_t* vals = nullptr;
   const uint32_t* scan_perm = nullptr;
   const uint32_t* scan_limit = nullptr;
   const uint32_t scan_tiles = (gn + 1 + kScanTile - 1) / kScanTile;
   if (P.kind == VBX_MERGED) {
-    KeyT* k0 = reinterpret_cast<KeyT*>(S.pkeys0);
-    KeyT* k1 = reinterpret_cast<KeyT*>(F.pkeys1);
     k_point_bounds<<<std::min<unsigned int>(grid_for(gn, TB), x.sms * 4), TB, 0, s>>>(
         A, F.first_bits, F.sort_plan0, F.scan_status, scan_tiles + 1, S.d_state);
-    k_point_keys<KeyT><<<grid_for(gn, TB), TB, 0, s>>>(A, order, k0, F.pvals[0], S.d_state);
-    mk.mark(0);
+    ++tally.launches;
+    k_point_keys<<<grid_for(gn, TB), TB, 0, s>>>(A, order, S.pkeys0, F.pvals[0], S.d_state);
+    ++tally.launches;
+    tally.mark(kStagePointKeys);
     // the bits in use are known on the device only (ScanState::key_bits): passes beyond them exit at once
-    if (int rc = own_sort<KeyT>(c, x, 0, k0, F.pvals[0], k1, F.pvals[1], &A->n, 0, n, 8 * (int)sizeof(KeyT), true,
-                                launches, &S.d_state->key_bits, /*plan_cleared=*/true)) {
+    if (int rc = own_sort(c, x, 0, S.pkeys0, F.pvals[0], F.pkeys1, F.pvals[1], &A->n, 0, n, 64, true, tally,
+                          &S.d_state->key_bits, /*plan_cleared=*/true)) {
       return rc;
     }
-    keys = k0;
-    vals = F.pvals[0];
-    mk.mark(1);
-    k_heads<KeyT><<<grid_for((uint64_t)gn + 1, TB), TB, 0, s>>>(A, keys, vals, c->order_inv, S.head_list, F.big_list,
-                                                                F.first_bits, S.cnt, S.d_state);
+    tally.mark(kStagePointSort);
+    k_heads<<<grid_for((uint64_t)gn + 1, TB), TB, 0, s>>>(A, S.pkeys0, F.pvals[0], c->order_inv, S.head_list, F.big_list,
+                                                          F.first_bits, S.cnt, S.d_state);
+    ++tally.launches;
     // The reference's bundle order (ray_list[rank] = bundle id, vbx_order.cuh) is one thread block's work
     // and the fold (k_merge) does not need it: the two run side by side.  (With stage profiling on they
     // run one after the other so that each gets its own time.)
-    cudaStream_t so = mk.on ? s : F.side;
+    cudaStream_t so = tally.on ? s : F.side;
     if (so != s) {
       VBX_CUDA(c, cudaEventRecord(F.ev_fork, s));
       VBX_CUDA(c, cudaStreamWaitEvent(so, F.ev_fork, 0));
     }
-    if (int rc = launch_bundle_order<KeyT>(c, x, so, P.n, keys, vals)) return rc;
+    if (int rc = launch_bundle_order(c, x, so, P.n, tally)) return rc;
     if (so != s) VBX_CUDA(c, cudaEventRecord(F.ev_join, so));
-    mk.mark(12);
-    k_merge<KeyT><<<x.sms * 4, 192, 0, s>>>(A, keys, vals, S.head_list, F.big_list, S.ray_p, S.ray_a, S.ray_c, S.cnt,
-                                            S.d_state);
-    mk.mark(8);
-    *launches += 8;
+    tally.mark(kStageBundleOrder);
+    k_merge<<<x.sms * 4, 192, 0, s>>>(A, S.pkeys0, F.pvals[0], S.head_list, F.big_list, S.ray_p, S.ray_a, S.ray_c, S.cnt,
+                                      S.d_state);
+    ++tally.launches;
+    tally.mark(kStageBundleMerge);
     if (!P.single_walk) {
       // the bundle count is only known on the device: launch for the worst case (every
       // point its own bundle); surplus threads exit on the first load
-      k_rays_count<KeyT><<<grid_for(gn, 128), 128, 0, s>>>(A, tab, order, keys, S.head_list, S.ray_p, S.ray_a, S.ray_c,
-                                                           S.cnt, c->set_start, c->set_observed, S.d_state);
-      *launches += 1;
+      k_rays_count<<<grid_for(gn, 128), 128, 0, s>>>(A, tab, order, S.pkeys0, S.head_list, S.ray_p, S.ray_a, S.ray_c,
+                                                     S.cnt, c->set_start, c->set_observed, S.d_state);
+      ++tally.launches;
     }
     if (so != s) VBX_CUDA(c, cudaStreamWaitEvent(s, F.ev_join, 0));
     // record offsets in RANK order: off[rank] = sum of cnt[ray_list[r]] over r < rank
     scan_perm = S.ray_list;
     scan_limit = &S.d_state->n_ray_list;
   } else {
-    k_rays_count<KeyT><<<grid_for((uint64_t)gn + 1, 128), 128, 0, s>>>(A, tab, order, keys, S.head_list, S.ray_p, S.ray_a,
-                                                                       S.ray_c, S.cnt, c->set_start, c->set_observed,
-                                                                       S.d_state);
-    *launches += 1;
+    k_rays_count<<<grid_for((uint64_t)gn + 1, 128), 128, 0, s>>>(A, tab, order, S.pkeys0, S.head_list, S.ray_p, S.ray_a,
+                                                                 S.ray_c, S.cnt, c->set_start, c->set_observed,
+                                                                 S.d_state);
+    ++tally.launches;
   }
-  mk.mark(2);
+  tally.mark(kStageRayCount);
   {
     // record offsets; the scan's last position also settles the call's update count (total_found, total_updates,
     // kErrUpdatesFull: too many for one pass; nothing downstream runs on a call that failed)
@@ -2367,23 +2328,21 @@ static int front_half(vbx_ctx* c, const ScanRoute& x, const ScanParams& P, const
     k_exclusive_scan<<<std::min<uint32_t>(scan_tiles, x.sms * 4), kSortThreads, 0, s>>>(
         S.cnt, scan_perm, scan_limit, S.off, &A->n_scan, 0u, F.scan_status + 1, F.scan_status, &S.d_state->total_found,
         &S.d_state->total_updates, &S.d_state->error, (unsigned long long)c->max_updates, kErrUpdatesFull);
+    ++tally.launches;
   }
-  mk.mark(3);
-  *launches += 1;
+  tally.mark(kStageScan);
   if (traced_in_front(P)) {
     // the Merged trace needs nothing of the map: it ends the front half, so the walk stage (submission
     // order) is left with k_assign's block creation
-    launch_trace<KeyT>(x, keys);
-    mk.mark(5);
-    *launches += 1;
+    launch_trace(x, tally);
+    tally.mark(kStageRayEmit);
   }
-  *keys_out = keys;
   return VBX_OK;
 }
 
 // update-record sort + the apply kernels.  cap: a pipelined scan's graph is being captured.  given: the records'
 // values are ordinals into these arrays, not ray ids (debug_apply)
-static int sort_and_apply(vbx_ctx* c, const ScanRoute& x, Marks& mk, uint64_t* launches, const Capture* cap,
+static int sort_and_apply(vbx_ctx* c, const ScanRoute& x, Tally& tally, const Capture* cap,
                           const GivenRecords* given = nullptr) {
   ScanRoute r = x;
   const vbx_ctx::ScratchSet& S = x.S;
@@ -2402,9 +2361,8 @@ static int sort_and_apply(vbx_ctx* c, const ScanRoute& x, Marks& mk, uint64_t* l
       VBX_CUDA(c, cudaStreamWaitEvent(cap->sort, cap->prev_sorted, cudaEventWaitExternal));
       r.s = cap->sort;
     }
-    if (int rc = own_sort<uint32_t>(c, r, 1, S.ckeys[0], S.cvals[0], S.ckeys[1], S.cvals[1], &S.d_state->total_updates,
-                                     0, c->record_hint, key_bits, false, launches, &S.d_state->rec_key_bits,
-                                     /*plan_cleared=*/true)) {
+    if (int rc = own_sort(c, r, 1, S.ckeys[0], S.cvals[0], S.ckeys[1], S.cvals[1], &S.d_state->total_updates, 0,
+                          c->record_hint, key_bits, false, tally, &S.d_state->rec_key_bits, /*plan_cleared=*/true)) {
       return rc;
     }
     rv.keys[0] = S.ckeys[0];
@@ -2427,7 +2385,8 @@ static int sort_and_apply(vbx_ctx* c, const ScanRoute& x, Marks& mk, uint64_t* l
   } else {
     k_apply_prep<false><<<x.sms * 8, 256, 0, s>>>(S.d_args, tab, rv, S.ray_a, S.ray_c, lr, S.d_state, GivenRecords{});
   }
-  mk.mark(6);
+  ++tally.launches;
+  tally.mark(kStageUpdateSort);
   if (cap) {
     // pipelined submission: the apply kernel runs behind the previous scan's apply, so the next scan's
     // ray walk can start while this scan's voxels are still being written
@@ -2438,35 +2397,34 @@ static int sort_and_apply(vbx_ctx* c, const ScanRoute& x, Marks& mk, uint64_t* l
     s = cap->apply;
   }
   k_apply<<<x.sms * 8, 32 * kApplyWarps, 0, s>>>(S.d_args, tab, rv, lr, S.d_state);
+  ++tally.launches;
   if (cap) VBX_CUDA(c, cudaEventRecordWithFlags(cap->applied, s, cudaEventRecordExternal));
-  mk.mark(7);
-  *launches += 2;
+  tally.mark(kStageApply);
   return VBX_OK;
 }
 
 // emitted: the front half has already written this call's update records (traced_in_front, one pass); the
 // passes of apply_in_passes trace their own rank window here.
-template <typename KeyT>
-static int back_half(vbx_ctx* c, const ScanRoute& x, const ScanParams& P, const KeyT* keys, bool emitted, Marks& mk,
-                     uint64_t* launches, const Capture* cap = nullptr) {
+static int back_half(vbx_ctx* c, const ScanRoute& x, const ScanParams& P, bool emitted, Tally& tally,
+                     const Capture* cap = nullptr) {
   cudaStream_t s = x.s;
   const vbx_ctx::ScratchSet& S = x.S;
   const Tables tab = scan_tables(c, S);
   if (!emitted) {
     if (traced_in_front(P)) {
-      launch_trace<KeyT>(x, keys);
+      launch_trace(x, tally);
     } else {
-      k_rays_emit<KeyT><<<grid_for(c->max_points, 128), 128, 0, s>>>(S.d_args, tab, keys, S.ray_list, S.head_list, S.ray_p,
-                                                                     S.cnt, S.off, S.ckeys[0], S.cvals[0], S.d_state);
+      k_rays_emit<<<grid_for(c->max_points, 128), 128, 0, s>>>(S.d_args, tab, S.pkeys0, S.ray_list, S.head_list, S.ray_p,
+                                                               S.cnt, S.off, S.ckeys[0], S.cvals[0], S.d_state);
+      ++tally.launches;
     }
-    mk.mark(5);
-    *launches += 1;
+    tally.mark(kStageRayEmit);
   }
   k_assign<<<1, kAssignThreads, 0, s>>>(tab, S.blocks, S.d_args, c->d_nblocks, S.sort_plan1, S.d_state);
+  ++tally.launches;
   c->nb_cur ^= 1;
-  mk.mark(4);
-  *launches += 1;
-  return sort_and_apply(c, x, mk, launches, cap);
+  tally.mark(kStageAssign);
+  return sort_and_apply(c, x, tally, cap);
 }
 
 static void fill_args(const vbx_ctx* c, const ScanParams& P, const float* xyz, const uint8_t* rgba, ScanArgs* a) {
@@ -2494,8 +2452,7 @@ int alloc_scan_args(vbx_ctx* c, vbx_ctx::ScratchSet& S) {
 }
 
 // The back half of a call whose K exceeds max_updates_per_pass, in passes (see integrate_device).
-template <typename KeyT>
-static int apply_in_passes(vbx_ctx* c, const ScanRoute& x, ScanArgs a, const KeyT* keys, Marks& mk, uint64_t* launches) {
+static int apply_in_passes(vbx_ctx* c, const ScanRoute& x, ScanArgs a, Tally& tally, uint32_t* passes) {
   cudaStream_t s = x.s;
   const uint32_t n = a.P.n;
   std::vector<uint32_t> off(n + 1);
@@ -2520,7 +2477,7 @@ static int apply_in_passes(vbx_ctx* c, const ScanRoute& x, ScanArgs a, const Key
     if (off[hi] > off[lo]) ranges.emplace_back(lo, hi);
     lo = hi;
   }
-  uint32_t passes = 0;
+  *passes = (uint32_t)ranges.size();
   for (const auto& r : ranges) {
     const uint32_t lo = r.first, hi = r.second;
     const unsigned long long kp = (unsigned long long)off[hi] - off[lo];
@@ -2531,12 +2488,17 @@ static int apply_in_passes(vbx_ctx* c, const ScanRoute& x, ScanArgs a, const Key
     VBX_CUDA(c, cudaStreamSynchronize(s));  // (the previous pass has read its arguments)
     if (int rc = upload_args(c, x, a)) return rc;
     k_pass_begin<<<1, 1, 0, s>>>(x.S.d_state, kp);
-    *launches += 1;
-    if (int rc = back_half<KeyT>(c, x, a.P, keys, /*emitted=*/false, mk, launches)) return rc;
-    ++passes;
+    ++tally.launches;
+    if (int rc = back_half(c, x, a.P, /*emitted=*/false, tally)) return rc;
   }
-  c->last_passes = passes;
   return VBX_OK;
+}
+
+// ScanParams::single_walk: a ray's update count is known from its DDA set-up alone (not Fast, no
+// anti-grazing).  Otherwise the front half walks the rays to count them, and that walk creates blocks (and
+// Fast's walk reads its approximate sets), so such scans cannot be pipelined (integrate_async).
+static bool single_walk(const vbx_tsdf_config& cfg, int kind) {
+  return kind != VBX_FAST && !(kind == VBX_MERGED && cfg.enable_anti_grazing);
 }
 
 static void fill_params(vbx_ctx* c, int kind, const float q[4], const float t[3], uint32_t n, int freespace,
@@ -2588,7 +2550,7 @@ static void fill_params(vbx_ctx* c, int kind, const float q[4], const float t[3]
   P.emit_lo = 0;
   P.emit_hi = 0xffffffffu;
   P.emit_base = 0;
-  P.single_walk = (kind != VBX_FAST && !(kind == VBX_MERGED && cfg.enable_anti_grazing)) ? 1 : 0;
+  P.single_walk = single_walk(cfg, kind) ? 1 : 0;
 }
 
 int integrate_device(vbx_ctx* c, const ScanRoute& x, int kind, const float q[4], const float t[3], const float* d_xyz,
@@ -2601,7 +2563,6 @@ int integrate_device(vbx_ctx* c, const ScanRoute& x, int kind, const float q[4],
   const vbx_ctx::FrontLane& F = x.F;
   const vbx_tsdf_config& cfg = c->cfg;
   std::memset(c->counters, 0, sizeof(c->counters));
-  uint64_t launches = 0;
 
   ScanParams P;
   fill_params(c, kind, q, t, n, freespace, P);
@@ -2618,65 +2579,76 @@ int integrate_device(vbx_ctx* c, const ScanRoute& x, int kind, const float q[4],
   fill_args(c, P, d_xyz, d_rgba, &a);
   if (int rc = upload_args(c, x, a)) return rc;
   const int TB = 256;
-  Marks mk{c, s, x.marks};
-  mk.begin();
+  Tally tally{c, s, x.marks};
+  tally.begin();
 
   const uint32_t* order = nullptr;
   if (cfg.integration_order_mode == 1) {
     // SortedThreadSafeIndex: ascending |p|^2 (stable here; std::sort leaves ties unspecified)
     k_sqnorm_keys<<<grid_for(n, TB), TB, 0, s>>>(n, d_xyz, S.pkeys0, F.pvals[0]);
-    if (int rc = own_sort<uint64_t>(c, x, 0, S.pkeys0, F.pvals[0], F.pkeys1, F.pvals[1], nullptr, n, n, 64, true, &launches)) {
-      return rc;
-    }
+    ++tally.launches;
+    if (int rc = own_sort(c, x, 0, S.pkeys0, F.pvals[0], F.pkeys1, F.pvals[1], nullptr, n, n, 64, true, tally)) return rc;
     VBX_CUDA(c, cudaMemcpyAsync(c->order, F.pvals[0], n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
     k_invert_order<<<grid_for(n, TB), TB, 0, s>>>(n, c->order, c->order_inv);
+    ++tally.launches;
     order = c->order;
-    launches += 2;
   }
 
-  const uint64_t* keys64 = nullptr;
-  if (int rc = front_half<uint64_t>(c, x, P, order, mk, &launches, &keys64)) return rc;
+  if (int rc = front_half(c, x, P, order, tally)) return rc;
   // own sort: K stays on the device, the whole call is enqueued without a host round trip
-  if (int rc = back_half<uint64_t>(c, x, P, keys64, traced_in_front(P), mk, &launches)) return rc;
+  if (int rc = back_half(c, x, P, traced_in_front(P), tally)) return rc;
   VBX_CUDA(c, cudaEventRecord(c->ev1, s));
   VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));
   const ScanState& h = *S.h_state;
   const uint32_t blocks_before = c->n_blocks;
   const bool chunked = h.error == kErrUpdatesFull;
+  uint32_t passes = 1;
   if (chunked) {
     // More update records than one pass holds.  Nothing was emitted or applied; the per-ray
     // tables, counts and offsets of the front half stand.  Apply the call in passes over
     // contiguous ray-slot ranges: every voxel still sees its updates in ray-rank order, so
     // the result is the one-pass result bit for bit.
-    if (int rc = apply_in_passes<uint64_t>(c, x, a, keys64, mk, &launches)) return rc;
+    if (int rc = apply_in_passes(c, x, a, tally, &passes)) return rc;
     VBX_CUDA(c, cudaEventRecord(c->ev1, s));
     VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
     VBX_CUDA(c, cudaStreamSynchronize(s));
   }
   if (int rc = check_state_errors(c, h)) return rc;
   c->n_blocks = h.n_blocks;
-  const unsigned long long K = h.total_found;
   VBX_CUDA(c, cudaGetLastError());
   VBX_CUDA(c, cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
-  mk.collect();
-  c->launches += launches;
-  c->counters[0] = h.n_rays;
-  if (kind == VBX_MERGED) c->bundle_hint = std::max(h.n_rays, h.n_clear_rays);
-  c->counters[1] = h.n_clear_rays;
-  c->counters[2] = K;
-  if (K) c->record_hint = K;
-  c->counters[3] = h.n_voxels;
-  c->counters[4] = h.n_touched;
-  c->counters[5] = chunked ? (uint64_t)(c->n_blocks - blocks_before) : (uint64_t)h.n_new;
-  c->counters[11] = chunked ? c->last_passes : 1;
-  c->counters[9] = h.n_refold;
-  c->counters[10] = h.refold_members;
-  c->counters[12] = h.key_bits;
-  c->counters[6] = (kind == VBX_MERGED) ? h.n_valid_points : (uint64_t)h.n_rays + h.n_clear_rays;
-  c->counters[7] = launches;
-  for (int i = 0; i < kApplyPaths; ++i) c->apply_paths[i] = h.apply_paths[i];
+  tally.collect();
+  c->launches += tally.launches;
+  report_scan(c, h, kind, tally.launches, passes, chunked ? (uint64_t)(c->n_blocks - blocks_before) : (uint64_t)h.n_new);
   return VBX_OK;
+}
+
+static void report_apply_paths(vbx_ctx* c, const ScanState& h) {
+  for (int i = 0; i < kApplyPaths; ++i) c->apply_paths[i] = h.apply_paths[i];
+}
+
+// The status block of a synchronous call (integrate_device) or a collected asynchronous scan (harvest_async)
+void report_scan(vbx_ctx* c, const ScanState& h, int kind, uint64_t launches, uint64_t passes,
+                 uint64_t blocks_allocated) {
+  uint64_t* cnt = c->counters;
+  std::memset(cnt, 0, sizeof(c->counters));
+  cnt[kCntRays] = h.n_rays;
+  cnt[kCntClearRays] = h.n_clear_rays;
+  cnt[kCntUpdates] = h.total_found;
+  cnt[kCntVoxels] = h.n_voxels;
+  cnt[kCntBlocksTouched] = h.n_touched;
+  cnt[kCntBlocksAllocated] = blocks_allocated;
+  cnt[kCntValidPoints] = kind == VBX_MERGED ? h.n_valid_points : (uint64_t)h.n_rays + h.n_clear_rays;
+  cnt[kCntLaunches] = launches;
+  cnt[kCntRefoldedBundles] = h.n_refold;
+  cnt[kCntRefoldedPoints] = h.refold_members;
+  cnt[kCntPasses] = passes;
+  cnt[kCntBundleKeyBits] = h.key_bits;
+  // (vbx_get_counters adds the context's totals)
+  if (h.total_found) c->record_hint = h.total_found;
+  if (kind == VBX_MERGED && !(h.error & kFatalErrors)) c->bundle_hint = std::max(h.n_rays, h.n_clear_rays);
+  report_apply_paths(c, h);
 }
 
 // ------------------------------------------------------------- asynchronous submission
@@ -2712,8 +2684,7 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
                     {c->cap_ev[2], c->cap_ev[3]}};
   const ScanRoute front{S, F, F.stream, sms, false}, walk{S, F, c->stream_e, sms, false};
   cudaStream_t o = S.stream;
-  uint64_t launches = 0;
-  Marks mk{c, F.stream, false};
+  Tally tally{c, F.stream, false};  // (the graph's kernel nodes are counted below)
   auto enqueue = [&]() -> int {
     VBX_CUDA(c, cudaMemcpyAsync(S.d_args, S.h_args, sizeof(ScanArgs), cudaMemcpyHostToDevice, o));
     VBX_CUDA(c, cudaStreamWaitEvent(o, S.copy_done, cudaEventWaitExternal));  // a host cloud's copy
@@ -2723,8 +2694,7 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
     VBX_CUDA(c, cudaStreamWaitEvent(F.stream, c->cap_ev[0], 0));
     VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), F.stream));
     if (c->timeline) VBX_CUDA(c, cudaEventRecordWithFlags(S.front_start, F.stream, cudaEventRecordExternal));
-    const uint64_t* keys64 = nullptr;
-    if (int rc = front_half<uint64_t>(c, front, P, nullptr, mk, &launches, &keys64)) return rc;
+    if (int rc = front_half(c, front, P, nullptr, tally)) return rc;
     VBX_CUDA(c, cudaEventRecordWithFlags(F.done, F.stream, cudaEventRecordExternal));
     if (c->timeline) VBX_CUDA(c, cudaEventRecordWithFlags(S.front_done, F.stream, cudaEventRecordExternal));
     // ---- walk, record sort and apply (sort_and_apply hands off between their streams)
@@ -2736,8 +2706,7 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
     // every scan queued behind it then skips its back half, and the host redoes all of them
     // synchronously, in order, from the retained inputs (recover_async, vbx_capi.cu).
     k_back_begin<<<1, 1, 0, c->stream_e>>>(S.d_state, c->d_hold);
-    launches += 1;
-    if (int rc = back_half<uint64_t>(c, walk, P, keys64, traced_in_front(P), mk, &launches, &cap)) return rc;
+    if (int rc = back_half(c, walk, P, traced_in_front(P), tally, &cap)) return rc;
     VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, cap.apply));
     // every stream of the capture joins its origin
     const cudaStream_t joined[4] = {F.stream, c->stream_e, c->stream_s, c->stream};
@@ -2756,6 +2725,7 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
   // and the nodes whose launch shape follows the scan or the hints.
   cudaGraphNode_t point_sort = nullptr, record_sort = nullptr, order = nullptr;
   cudaKernelNodeParams pp = {}, rp = {}, op = {};
+  uint64_t launches = 0;
   if (rc == VBX_OK) {
     const int walk_prio = std::min(c->prio_lo, c->prio_hi + 1), sort_prio = std::min(c->prio_lo, c->prio_hi + 2);
     size_t nn = 0;
@@ -2769,10 +2739,11 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
           cudaGraphKernelNodeGetParams(nd, &kp) != cudaSuccess) {
         continue;
       }
+      ++launches;
       cudaLaunchAttributeValue prio = {};
       prio.priority = c->prio_lo;
       // (the Merged trace, k_rays_emit_warp, is a front-half node: it keeps the front priority)
-      if (kp.func == (void*)k_back_begin || kp.func == (void*)k_rays_emit<uint64_t> || kp.func == (void*)k_assign) {
+      if (kp.func == (void*)k_back_begin || kp.func == (void*)k_rays_emit || kp.func == (void*)k_assign) {
         prio.priority = walk_prio;
       } else if (kp.func == (void*)k_sort<uint32_t> || kp.func == (void*)k_apply_prep<false>) {
         prio.priority = sort_prio;
@@ -2870,8 +2841,7 @@ int integrate_async(vbx_ctx* c, const ScanRoute& sync, int kind, const float q[4
   if (kind < VBX_SIMPLE || kind > VBX_FAST) return fail(c, VBX_E_INVALID, "Unknown TSDF integrator type");
   if (n64 > c->max_points) return fail(c, VBX_E_CAPACITY, "cloud larger than max_points_per_scan");
   const vbx_tsdf_config& cfg = c->cfg;
-  const bool overlappable = kind != VBX_FAST && !(kind == VBX_MERGED && cfg.enable_anti_grazing) &&
-                            cfg.integration_order_mode == 0 && n64 > 0;
+  const bool overlappable = single_walk(cfg, kind) && cfg.integration_order_mode == 0 && n64 > 0;
   if (!overlappable) {
     // configurations whose front half touches the map or the Fast integrator's sets run in order
     if (int rc = drain_async(c)) return rc;
@@ -3015,7 +2985,7 @@ int debug_sort(vbx_ctx* c, const void* keys, int key_bytes, uint32_t n, int key_
   const vbx_ctx::ScratchSet& S = x.S;
   const vbx_ctx::FrontLane& F = x.F;
   cudaStream_t s = x.s;
-  uint64_t launches = 0;
+  Tally tally{c, s, false};
   if (key_bytes == 4) {
     if (n > c->max_updates) return fail(c, VBX_E_CAPACITY, "debug_sort: n > max_updates_per_pass");
     VBX_CUDA(c, cudaMemcpyAsync(S.ckeys[0], keys, (size_t)n * 4, cudaMemcpyHostToDevice, s));
@@ -3023,8 +2993,8 @@ int debug_sort(vbx_ctx* c, const void* keys, int key_bytes, uint32_t n, int key_
     VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), s));
     const unsigned long long nn = n;
     VBX_CUDA(c, cudaMemcpyAsync(&S.d_state->total_updates, &nn, sizeof(nn), cudaMemcpyHostToDevice, s));
-    if (int rc = own_sort<uint32_t>(c, x, 1, S.ckeys[0], S.cvals[0], S.ckeys[1], S.cvals[1], &S.d_state->total_updates,
-                                     0, n, key_bits, true, &launches)) {
+    if (int rc = own_sort(c, x, 1, S.ckeys[0], S.cvals[0], S.ckeys[1], S.cvals[1], &S.d_state->total_updates, 0, n,
+                          key_bits, true, tally)) {
       return rc;
     }
     VBX_CUDA(c, cudaMemcpyAsync(keys_out, S.ckeys[0], (size_t)n * 4, cudaMemcpyDeviceToHost, s));
@@ -3033,8 +3003,7 @@ int debug_sort(vbx_ctx* c, const void* keys, int key_bytes, uint32_t n, int key_
     if (n > c->max_points) return fail(c, VBX_E_CAPACITY, "debug_sort: n > max_points_per_scan");
     VBX_CUDA(c, cudaMemcpyAsync(S.pkeys0, keys, (size_t)n * 8, cudaMemcpyHostToDevice, s));
     k_iota<<<c->grid_sms, 256, 0, s>>>(F.pvals[0], n);
-    if (int rc = own_sort<uint64_t>(c, x, 0, S.pkeys0, F.pvals[0], F.pkeys1, F.pvals[1], nullptr, n, n, key_bits, true,
-                                     &launches)) {
+    if (int rc = own_sort(c, x, 0, S.pkeys0, F.pvals[0], F.pkeys1, F.pvals[1], nullptr, n, n, key_bits, true, tally)) {
       return rc;
     }
     VBX_CUDA(c, cudaMemcpyAsync(keys_out, S.pkeys0, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
@@ -3135,15 +3104,14 @@ int debug_apply(vbx_ctx* c, const int32_t* idx3, uint32_t nb, uint64_t n, const 
     VBX_CUDA(c, cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
     VBX_CUDA(c, cudaStreamSynchronize(s));
     if (bad) return fail(c, VBX_E_INVALID, "debug_apply: a block is not in the TSDF layer");
-    Marks mk{c, s, x.marks};
-    uint64_t launches = 0;
+    Tally tally{c, s, x.marks};
     const GivenRecords given{d_sdf, d_w, d_col};
-    if (int rc = sort_and_apply(c, x, mk, &launches, nullptr, &given)) return rc;
+    if (int rc = sort_and_apply(c, x, tally, nullptr, &given)) return rc;
     VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
     VBX_CUDA(c, cudaStreamSynchronize(s));
     VBX_CUDA(c, cudaGetLastError());
     if (int rc = check_state_errors(c, *S.h_state)) return rc;
-    for (int i = 0; i < 16; ++i) c->apply_paths[i] = i < kApplyPaths ? S.h_state->apply_paths[i] : 0;
+    report_apply_paths(c, *S.h_state);
     if (paths) std::memcpy(paths, c->apply_paths, sizeof(c->apply_paths));
     return VBX_OK;
   };
