@@ -14,6 +14,7 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 
 from oracle import pyoracle as po  # noqa: E402
+from tests import test_block_sizes_gpu as tb  # noqa: E402
 from tests import test_esdf_options_gpu as teo  # noqa: E402
 from tests import test_esdf_reference_gpu as te  # noqa: E402
 from tests import test_icp_cpu as tic  # noqa: E402
@@ -45,6 +46,8 @@ def cases():
         out[f"tsdf_ground_truth/{key}"] = lambda lib, k=key: tg.reference_side(k, lib)[1]
     for key in ti.PIN_KEYS:
         out[f"icp/{key}"] = lambda lib, k=key: ti.reference_side(k, lib)[2]
+    for key in tb.PIN_KEYS:
+        out[f"block_sizes/{key}"] = lambda lib, k=key: tb.reference_side(k, lib)[2]
     for name, fn in to.REFERENCE_CASES.items():
         out[f"oracle_pin/{name}"] = lambda lib, f=fn: _joined(f(lib))
     return out
@@ -55,7 +58,7 @@ def main():
     pinned = {}
     for key, fn in cases().items():
         pinned[key] = fn(ref)
-        if key.startswith("icp/refine"):
+        if key.startswith("icp/refine") or key.startswith("block_sizes/icp/"):
             same = fn(port)["map"] == pinned[key]["map"]   # the restatement's ICP is compared at 1e-5, not bit for bit
         elif key == "mesh/mc_tables":
             same = True                                     # the restatement owns no copy of the table

@@ -62,6 +62,10 @@ __global__ void k_rebuild_hash(Tables tab, uint32_t n_blocks) {
 
 static inline unsigned int grid_for(uint64_t n, int block) { return (unsigned int)((n + block - 1) / block); }
 
+// The block transfer kernels take the block number from blockIdx.y, which is capped at 65,535: larger
+// batches are launched in slices of at most that many blocks.
+static constexpr uint64_t kMaxGridY = 65535;
+
 // The block hash rebuilt from slot_key: after removals, and after a call that ran out of pool slots
 // (its surplus hash entries have no slot and must not be found by later calls).
 int rebuild_hash(vbx_ctx* c) {
@@ -223,14 +227,17 @@ int upload_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, const 
     VBX_CUDA(c, cudaMemcpyAsync(c->mirror_dev, static_cast<const char*>(voxels) + at * bbytes, k * bbytes,
                                 cudaMemcpyHostToDevice, s));
     if (updated_bits) VBX_CUDA(c, cudaMemcpyAsync(d_upd, updated_bits + at, k, cudaMemcpyHostToDevice, s));
-    const dim3 grid(grid_for((uint64_t)wpv * c->vox_per_block, 256), (unsigned int)k);
-    k_scatter_blocks<<<grid, 256, 0, s>>>(layer, serialized, static_cast<const uint32_t*>(c->mirror_dev),
-                                          reinterpret_cast<const int32_t*>(S.cnt) + at, (uint32_t)k,
-                                          (uint32_t)c->vox_per_block, pool, updated_bits ? d_upd : nullptr, flags,
-                                          layer == VBX_LAYER_ESDF ? c->tab.slot_has_esdf : nullptr);
+    for (uint64_t b0 = 0; b0 < k; b0 += kMaxGridY) {
+      const uint64_t kb = std::min<uint64_t>(kMaxGridY, k - b0);
+      const dim3 grid(grid_for((uint64_t)wpv * c->vox_per_block, 256), (unsigned int)kb);
+      k_scatter_blocks<<<grid, 256, 0, s>>>(
+          layer, serialized, reinterpret_cast<const uint32_t*>(static_cast<const char*>(c->mirror_dev) + b0 * bbytes),
+          reinterpret_cast<const int32_t*>(S.cnt) + at + b0, (uint32_t)kb, (uint32_t)c->vox_per_block, pool,
+          updated_bits ? d_upd + b0 : nullptr, flags, layer == VBX_LAYER_ESDF ? c->tab.slot_has_esdf : nullptr);
+      VBX_CUDA(c, cudaGetLastError());
+    }
     VBX_CUDA(c, cudaStreamSynchronize(s));  // the staging buffer is reused by the next chunk
   }
-  VBX_CUDA(c, cudaGetLastError());
   return refresh_host_mirror(c);
 }
 
@@ -373,6 +380,19 @@ __global__ void k_gather_blocks(const uint4* __restrict__ pool, const uint32_t* 
   if (part == 0 && threadIdx.x == 0 && clear_mask) flags[slot] &= (uint8_t)~clear_mask;
 }
 
+// The same for payloads that are not a multiple of 16 B (one-voxel blocks: 12 B TSDF, 20 B ESDF): one
+// thread per output word, consecutive threads on consecutive words
+__global__ void k_gather_words(const uint32_t* __restrict__ pool, const uint32_t* __restrict__ slots, uint32_t m,
+                               uint32_t words_per_block, uint32_t* __restrict__ out, uint8_t* __restrict__ flags,
+                               uint8_t clear_mask) {
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= (uint64_t)m * words_per_block) return;
+  const uint32_t b = (uint32_t)(g / words_per_block), i = (uint32_t)(g % words_per_block);
+  const uint32_t slot = slots[b];
+  out[g] = __ldcs(pool + (size_t)slot * words_per_block + i);
+  if (i == 0 && clear_mask) flags[slot] &= (uint8_t)~clear_mask;
+}
+
 int mirror_updated(vbx_ctx* c, int layer, int updated_mask, int clear_mask, int32_t* idx3, void* voxels,
                    uint8_t* updated_bits, uint64_t cap, uint64_t* n, int serialized) {
   cudaStream_t s = c->stream;
@@ -414,7 +434,6 @@ int mirror_updated(vbx_ctx* c, int layer, int updated_mask, int clear_mask, int3
   const size_t m = items.size();
   const size_t raw_bytes = ((layer == VBX_LAYER_TSDF) ? sizeof(TsdfVoxel) : sizeof(EsdfVoxel)) * c->vox_per_block;
   const size_t bbytes = payload_bytes(c, layer, serialized);
-  if (raw_bytes % 16 != 0) return fail(c, VBX_E_STATE, "block payload is not a multiple of 16 bytes");
   if (int rc = ensure_staging(c, m * bbytes, m)) return rc;
   std::vector<uint32_t> slots(m);
   for (size_t i = 0; i < m; ++i) {
@@ -431,15 +450,26 @@ int mirror_updated(vbx_ctx* c, int layer, int updated_mask, int clear_mask, int3
                                                : reinterpret_cast<const char*>(c->tab.esdf);
   if (serialized) {
     const uint32_t tpv = (layer == VBX_LAYER_TSDF) ? 3u : 1u;
-    const dim3 grid(grid_for((uint64_t)tpv * c->vox_per_block, 256), (unsigned int)m);
-    k_serialize_blocks<<<grid, 256, 0, s>>>(layer, reinterpret_cast<const uint32_t*>(pool), c->mirror_slots, (uint32_t)m,
-                                            (uint32_t)c->vox_per_block, static_cast<uint32_t*>(c->mirror_dev), flags,
-                                            (uint8_t)(clear_mask & 0x7f));
-  } else {
+    for (size_t b0 = 0; b0 < m; b0 += kMaxGridY) {
+      const size_t kb = std::min<size_t>(kMaxGridY, m - b0);
+      const dim3 grid(grid_for((uint64_t)tpv * c->vox_per_block, 256), (unsigned int)kb);
+      k_serialize_blocks<<<grid, 256, 0, s>>>(
+          layer, reinterpret_cast<const uint32_t*>(pool), c->mirror_slots + b0, (uint32_t)kb, (uint32_t)c->vox_per_block,
+          reinterpret_cast<uint32_t*>(static_cast<char*>(c->mirror_dev) + b0 * bbytes), flags,
+          (uint8_t)(clear_mask & 0x7f));
+      VBX_CUDA(c, cudaGetLastError());
+    }
+  } else if (raw_bytes % 16 == 0) {
     k_gather_blocks<<<(unsigned int)(m * 8), 256, 0, s>>>(reinterpret_cast<const uint4*>(pool), c->mirror_slots,
                                                            (uint32_t)m, (uint32_t)(raw_bytes / 16),
                                                            reinterpret_cast<uint4*>(c->mirror_dev), flags,
                                                            (uint8_t)(clear_mask & 0x7f));
+    VBX_CUDA(c, cudaGetLastError());
+  } else {
+    k_gather_words<<<grid_for((uint64_t)m * (raw_bytes / 4), 256), 256, 0, s>>>(
+        reinterpret_cast<const uint32_t*>(pool), c->mirror_slots, (uint32_t)m, (uint32_t)(raw_bytes / 4),
+        static_cast<uint32_t*>(c->mirror_dev), flags, (uint8_t)(clear_mask & 0x7f));
+    VBX_CUDA(c, cudaGetLastError());
   }
   // straight into the caller's buffer when it is page-locked (vbx_host_alloc / cudaHostRegister),
   // otherwise through the engine's page-locked staging buffer

@@ -106,7 +106,7 @@ struct ScanState {
   uint32_t key_bits;         // bits a bundle key uses
   uint32_t n_big;            // Merged: bundles of at least kBigBundle members (folded first)
   uint32_t merge_ticket;     // Merged: work hand-out counter of k_merge
-  uint32_t n_touch_ids;      // touched-block ids handed out (>= n_touched: ids lost to a race stay unused)
+  uint32_t n_touch_ids;      // touched-block ids handed out: one per block the call touches (vbx_hash.cuh)
   uint32_t rec_key_bits;     // bits an update-record key uses: voxel-in-block bits + bits of the touched ids
   uint32_t esdf_ticket[6];   // ESDF queue kernels: work hand-out counters, rotating like the queue counters ([0..2] raise, [3..5] lower)
   uint32_t tile_ticket;      // k_apply: record tiles of the short runs handed out
@@ -144,7 +144,7 @@ struct Tables {
 // zeroed once when it is allocated; k_assign clears the positions a call used.
 struct ScanBlocks {
   uint32_t* table;            // [mask + 1], a power of two >= 2 * cap
-  unsigned long long* keys;   // [cap] local id -> packed block index (0: an id lost to a race, a hole)
+  unsigned long long* keys;   // [cap] local id -> packed block index
   uint32_t* pos;              // [cap] local id -> its table position
   uint32_t mask;
   uint32_t cap;               // = Tables::touched_cap

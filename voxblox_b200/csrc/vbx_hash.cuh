@@ -57,72 +57,85 @@ __device__ __forceinline__ uint32_t find_block(const Tables& t, uint64_t key) {
   return 0xffffffffu;
 }
 
-// Blocks touched by the current call get dense ids 0, 1, 2, ... (update records are keyed by
-// (touched id, voxel in block): a handful of bits instead of a hash position).  The per-position
-// word packs (call id, touched id); the first toucher of a block in this call installs it with one
-// CAS.  A thread that loses the CAS race has drawn an id nobody uses: it is marked as a hole in
-// touched_list (0xffffffff) -- ids stay dense enough, n_touched counts the blocks exactly.
-__device__ __forceinline__ uint32_t touch_block(const Tables& t, uint32_t hp, uint32_t epoch, ScanState* st) {
-  unsigned long long* w = t.htouch + hp;
-  const unsigned long long cur = *reinterpret_cast<volatile unsigned long long*>(w);
-  if ((uint32_t)(cur >> 32) == epoch) return (uint32_t)cur;
-  const uint32_t id = atomicAdd(&st->n_touch_ids, 1u);
-  if (id >= t.touched_cap) {
-    atomicOr(&st->error, kErrPoolFull);
-    return 0u;
-  }
-  const unsigned long long want = ((unsigned long long)epoch << 32) | id;
-  const unsigned long long old = atomicCAS(w, cur, want);
-  if (old == cur) {
-    t.touched_list[id] = hp;
-    atomicAdd(&st->n_touched, 1u);
-    return id;
-  }
-  t.touched_list[id] = 0xffffffffu;  // a hole
-  return (uint32_t)old;              // (only this call's walk writes these words: the winner carries this call's id)
-}
-
-// ------------------------------------------------------ scan-private block table
-// The local id of a block in the scan's private table (ScanBlocks), drawn from the same counter and installed
-// the same way as touch_block's ids, without reading the block hash: an id is drawn and its key written to
-// the block list first, then one CAS installs (id + 1) at a free position.  A reader that meets an occupied
-// position compares the key listed under its id (published before the CAS).  A thread whose key another
-// thread installed first leaves its drawn id as a hole (key 0; a block index packs to a non-zero key).
 __device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
   uint32_t v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
 
+__device__ __forceinline__ unsigned long long ld_acquire_gpu(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// An id word that a thread has claimed and not yet filled in: the thread that wins a block draws its id
+// only after its claim succeeded, so a race for a block's first touch draws ONE id, however many threads
+// take part.  (At voxels_per_side 1 every walk step is a new block and thousands of rays leave the sensor
+// together: drawing before the claim burnt an id per racing thread, ~100x the blocks a scan touches.)
+constexpr uint32_t kPendingId = 0xffffffffu;
+
+// Blocks touched by the current call get dense ids 0, 1, 2, ... (update records are keyed by
+// (touched id, voxel in block): a handful of bits instead of a hash position).  The per-position
+// word packs (call id, touched id); the first toucher of a block in this call claims the word with
+// one CAS (call id, kPendingId), draws the id and publishes it; the others wait for it.  Only this
+// call's walk writes these words, so n_touch_ids == n_touched.
+__device__ __forceinline__ uint32_t touch_block(const Tables& t, uint32_t hp, uint32_t epoch, ScanState* st) {
+  unsigned long long* w = t.htouch + hp;
+  const unsigned long long mine = (unsigned long long)epoch << 32;
+  unsigned long long cur = ld_acquire_gpu(w);
+  while ((uint32_t)(cur >> 32) != epoch) {
+    const unsigned long long old = atomicCAS(w, cur, mine | kPendingId);
+    if (old == cur) {
+      uint32_t id = atomicAdd(&st->n_touch_ids, 1u);
+      if (id < t.touched_cap) {
+        t.touched_list[id] = hp;
+        atomicAdd(&st->n_touched, 1u);
+      } else {
+        atomicOr(&st->error, kErrPoolFull);
+        id = 0u;  // (the call fails; the waiting threads must not spin on the claim)
+      }
+      atomicExch(w, mine | id);
+      return id;
+    }
+    cur = old;
+  }
+  while ((uint32_t)cur == kPendingId) cur = ld_acquire_gpu(w);  // another thread of this call claimed the block
+  return (uint32_t)cur;
+}
+
+// ------------------------------------------------------ scan-private block table
+// The local id of a block in the scan's private table (ScanBlocks), drawn from the same counter, without
+// reading the block hash.  The first thread to meet a free position claims it with one CAS (kPendingId),
+// draws an id, lists its key and position under it and then publishes id + 1 at the position.  A reader that
+// meets a claimed position waits for the id, then compares the key listed under it.  Every id drawn names a
+// block (ids drawn past the capacity raise kErrPoolFull and free the position again).
 __device__ inline uint32_t scan_block_id(const ScanBlocks& b, uint64_t key, ScanState* st) {
   uint32_t pos = hash64(key) & b.mask;
-  uint32_t drawn = 0xffffffffu;
-  for (uint32_t probe = 0; probe <= b.mask; ++probe) {
+  for (uint32_t probe = 0; probe <= b.mask;) {
     uint32_t v = ld_acquire_gpu(b.table + pos);
     if (v == 0u) {
-      if (drawn == 0xffffffffu) {
-        drawn = atomicAdd(&st->n_touch_ids, 1u);
-        if (drawn >= b.cap) {
+      v = atomicCAS(b.table + pos, 0u, kPendingId);
+      if (v == 0u) {
+        const uint32_t id = atomicAdd(&st->n_touch_ids, 1u);
+        if (id >= b.cap) {
           atomicOr(&st->error, kErrPoolFull);
+          atomicExch(b.table + pos, 0u);
           return 0xffffffffu;
         }
-        b.keys[drawn] = key;
+        b.keys[id] = key;
+        b.pos[id] = pos;
         __threadfence();  // the key is visible before the id can be found
+        atomicExch(b.table + pos, id + 1u);
+        return id;
       }
-      v = atomicCAS(b.table + pos, 0u, drawn + 1u);
-      if (v == 0u) {
-        b.pos[drawn] = pos;
-        return drawn;
-      }
-      __threadfence();  // (the winner's key was published before its CAS)
     }
-    if (*reinterpret_cast<volatile unsigned long long*>(b.keys + (v - 1u)) == key) {
-      if (drawn != 0xffffffffu) b.keys[drawn] = 0ull;  // a hole
-      return v - 1u;
-    }
+    while (v == kPendingId) v = ld_acquire_gpu(b.table + pos);
+    if (v == 0u) continue;  // (a claim that ran past the capacity was given back: try the position again)
+    if (*reinterpret_cast<volatile unsigned long long*>(b.keys + (v - 1u)) == key) return v - 1u;
     pos = (pos + 1u) & b.mask;
+    ++probe;
   }
-  if (drawn != 0xffffffffu) b.keys[drawn] = 0ull;
   atomicOr(&st->error, kErrHashFull);
   return 0xffffffffu;
 }

@@ -1257,7 +1257,7 @@ k_assign(Tables tab, ScanBlocks sb, const ScanArgs* __restrict__ A, uint32_t* __
       uint32_t touched = 0;
       for (uint32_t id0 = st->ids_resolved; id0 < n_ids; id0 += blockDim.x) {
         const uint32_t id = id0 + t;
-        const uint64_t key = id < n_ids ? sb.keys[id] : 0ull;  // (0: a hole)
+        const uint64_t key = id < n_ids ? sb.keys[id] : 0ull;
         bool created = false;
         uint32_t hp = 0xffffffffu;
         if (key != 0ull) {
