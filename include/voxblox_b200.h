@@ -71,7 +71,11 @@ typedef struct vbx_ctx vbx_ctx;
 /* POD mirror of TsdfIntegratorBase::Config, tsdf_integrator.h:56-89 (defaults there).
  * integration_order_mode: 0 = "mixed", 1 = "sorted" (integrator_utils.cc:5-15).
  * integrator_threads is accepted for API parity and ignored: the device applies
- * every voxel's updates in one fixed order (DESIGN.md, "update order"). */
+ * every voxel's updates in one fixed order (DESIGN.md, "update order").
+ * Fast only: max_integration_time_s <= 0 or NaN integrates no point of a call, as in the reference;
+ * a positive limit is wall-clock time and is not enforced.  clear_checks_every_n_frames counts the
+ * Fast calls of this context; the reference's counter is one static shared by every Fast integrator
+ * of the process (tsdf_integrator.cc:564). */
 typedef struct vbx_tsdf_config {
   float default_truncation_distance;
   float max_weight;
@@ -372,6 +376,10 @@ VBX_API int vbx_debug_apply(vbx_ctx* ctx, const int32_t* idx3, uint32_t n_blocks
 /* Counting the apply's paths costs a little on every call, so integrate calls count them only after
  * vbx_debug_count_apply_paths(ctx, 1) (off by default); vbx_debug_apply always counts. */
 VBX_API int vbx_debug_count_apply_paths(vbx_ctx* ctx, int enabled);
+/* Test hook for the Fast integrator: with enabled != 0 (off by default) later Fast calls walk their rays
+ * on one device thread in point order, which is the reference's one-thread schedule, so the approximate
+ * sets make the reference's decisions exactly.  Everything after that walk runs as usual.  Slow: for tests only. */
+VBX_API int vbx_debug_serial_fast(vbx_ctx* ctx, int enabled);
 /* How often each path of the apply ran in the last synchronous integrate call (summed over its passes),
  * the last collected asynchronous scan, or vbx_debug_apply (zero for calls made with counting off): [0] voxel runs longer than 32 updates (one
  * warp each) [1] ... cut short at rest (+T, max_weight) [2..4] 128-record steps decided in one go:

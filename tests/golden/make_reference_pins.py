@@ -17,6 +17,7 @@ from oracle import pyoracle as po  # noqa: E402
 from tests import test_block_sizes_gpu as tb  # noqa: E402
 from tests import test_esdf_options_gpu as teo  # noqa: E402
 from tests import test_esdf_reference_gpu as te  # noqa: E402
+from tests import test_fast_reference_gpu as tf  # noqa: E402
 from tests import test_icp_cpu as tic  # noqa: E402
 from tests import test_icp_gpu as ti  # noqa: E402
 from tests import test_merged_reference_gpu as tm  # noqa: E402
@@ -48,6 +49,9 @@ def cases():
         out[f"icp/{key}"] = lambda lib, k=key: ti.reference_side(k, lib)[2]
     for key in tb.PIN_KEYS:
         out[f"block_sizes/{key}"] = lambda lib, k=key: tb.reference_side(k, lib)[2]
+    for key in tf.PIN_KEYS:
+        # (reference_side primes the library's process-wide Fast reset counter first)
+        out[f"fast_reference/{key}"] = lambda lib, k=key: tf.reference_side(k, lib)[2]
     for name, fn in to.REFERENCE_CASES.items():
         out[f"oracle_pin/{name}"] = lambda lib, f=fn: _joined(f(lib))
     return out

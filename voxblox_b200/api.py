@@ -135,7 +135,7 @@ EXPORTS = ["vbx_create", "vbx_destroy", "vbx_last_error", "vbx_version", "vbx_ge
            "vbx_esdf_create", "vbx_esdf_update", "vbx_esdf_get_counters", "vbx_sync",
            "vbx_timer_start", "vbx_timer_stop_ms", "vbx_set_stage_profiling", "vbx_get_stage_ms",
            "vbx_host_alloc", "vbx_host_free", "vbx_host_copy_ms", "vbx_block_owner",
-           "vbx_debug_sort", "vbx_debug_scan", "vbx_debug_bundle_order", "vbx_debug_apply", "vbx_debug_apply_paths", "vbx_debug_count_apply_paths", "vbx_debug_async_timeline", "vbx_tsdf_integrate_async", "vbx_esdf_update_blocks", "vbx_esdf_set_max_distance",
+           "vbx_debug_sort", "vbx_debug_scan", "vbx_debug_bundle_order", "vbx_debug_apply", "vbx_debug_apply_paths", "vbx_debug_count_apply_paths", "vbx_debug_serial_fast", "vbx_debug_async_timeline", "vbx_tsdf_integrate_async", "vbx_esdf_update_blocks", "vbx_esdf_set_max_distance",
            "vbx_esdf_set_full_euclidean", "vbx_esdf_get_config", "vbx_esdf_add_robot_position", "vbx_esdf_clear", "vbx_mesh_generate", "vbx_mesh_download", "vbx_icp_run", "vbx_icp_run_device", "vbx_mirror_updated", "vbx_serialize_updated", "vbx_deserialize_blocks", "vbx_save_layer", "vbx_load_layer",
            "vbx_proto_encode_layer", "vbx_proto_encode_block", "vbx_proto_decode_block"]
 
@@ -179,6 +179,8 @@ def load_library():
     lib.vbx_debug_apply_paths.argtypes = [vp, vp]
     lib.vbx_debug_count_apply_paths.restype = i32
     lib.vbx_debug_count_apply_paths.argtypes = [vp, i32]
+    lib.vbx_debug_serial_fast.restype = i32
+    lib.vbx_debug_serial_fast.argtypes = [vp, i32]
     lib.vbx_esdf_get_counters.restype = i32
     lib.vbx_esdf_get_counters.argtypes = [vp, vp]
     lib.vbx_last_device_ms.restype = i32
@@ -618,6 +620,12 @@ class TsdfIntegratorBase:
         """Make later integrate calls count the apply's paths (vbx_debug_count_apply_paths; off by default)."""
         self._ctx.check(self._ctx.lib.vbx_debug_count_apply_paths(self._ctx.handle, int(bool(enabled))),
                         "vbx_debug_count_apply_paths")
+
+    def serialFast(self, enabled: bool = True) -> None:
+        """Make later Fast calls walk their rays on one thread in point order, the reference's one-thread
+        schedule (vbx_debug_serial_fast; off by default, for tests)."""
+        self._ctx.check(self._ctx.lib.vbx_debug_serial_fast(self._ctx.handle, int(bool(enabled))),
+                        "vbx_debug_serial_fast")
 
     def applyPaths(self) -> Dict[str, int]:
         """How often each arithmetic path of the apply ran in the last call (vbx_debug_apply_paths)."""

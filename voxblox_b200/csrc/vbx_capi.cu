@@ -376,10 +376,9 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
   if (int rc = init_bundle_order(c)) return rc;
   c->sort_tiles_cap[0] = (uint32_t)((np + kSortTile - 1) / kSortTile);
   c->sort_tiles_cap[1] = (uint32_t)((c->max_updates + kSortTile - 1) / kSortTile);
-  CK(dmalloc(&c->set_start, 1u << 20));
-  CK(dmalloc(&c->set_observed, 1u << 20));
-  CK(cudaMemsetAsync(c->set_start, 0, sizeof(unsigned long long) << 20, c->stream));
-  CK(cudaMemsetAsync(c->set_observed, 0, sizeof(unsigned long long) << 20, c->stream));
+  CK(dmalloc(&c->set_start, kApproxSetWords));
+  CK(dmalloc(&c->set_observed, kApproxSetWords));
+  if (int rc = init_fast_sets(c, c->stream)) return rc;
   CK(dmalloc(&c->d_nblocks, 2));
   CK(cudaMemsetAsync(c->d_nblocks, 0, 2 * sizeof(uint32_t), c->stream));
   CK(dmalloc(&c->d_hold, 1));
@@ -593,6 +592,14 @@ int vbx_debug_count_apply_paths(vbx_ctx* c, int enabled) {
   VBX_CUDA(c, cudaSetDevice(c->device));
   VBX_DRAIN(c);  // (scans already queued keep the setting they were submitted with)
   c->count_apply_paths = enabled != 0;
+  return VBX_OK;
+}
+
+int vbx_debug_serial_fast(vbx_ctx* c, int enabled) {
+  if (!c) return VBX_E_INVALID;
+  VBX_CUDA(c, cudaSetDevice(c->device));
+  VBX_DRAIN(c);
+  c->serial_fast = enabled != 0;
   return VBX_OK;
 }
 

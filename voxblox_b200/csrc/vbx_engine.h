@@ -24,6 +24,11 @@ namespace vbx {
 constexpr uint64_t kEmptyKey = ~0ull;
 constexpr uint64_t kInvalidPointKey = ~0ull;
 constexpr int kCoordBias = 1 << 20;  // block / voxel coordinates are packed 21 bits per axis
+// The Fast integrator's approximate sets, laid out as ApproxHashSet<20, 10000> (utils/approx_hash_array.h:75-179):
+// hash h lives in slot (h & kApproxSetMask) + offset; the offset moves on by one per reset, and the set is
+// cleared when it reaches kApproxSetResets.
+constexpr uint32_t kApproxSetMask = (1u << 20) - 1u, kApproxSetResets = 10000u;
+constexpr size_t kApproxSetWords = (1u << 20) + kApproxSetResets;
 // Internal bits of the per-slot flag bytes (never reported through the C-ABI):
 //   slot_updated bit 7: the slot holds an ESDF block only -- the TSDF layer has no block at this
 //     index (blocks allocated by EsdfIntegrator::addNewRobotPosition or uploaded into the ESDF layer).
@@ -202,10 +207,11 @@ struct vbx_ctx {
   size_t order_smem_bytes = 0;             // dynamic shared memory of k_bundle_order
   // tiles of the engine's own radix sorts (vbx_sort.cuh): [0] point keys, [1] update records
   uint32_t sort_tiles_cap[2] = {0, 0};
-  unsigned long long* set_start = nullptr;  // Fast integrator approximate sets
+  // the Fast integrator's approximate sets, kApproxSetWords each, and their slot offset (init_fast_sets)
+  unsigned long long* set_start = nullptr;
   unsigned long long* set_observed = nullptr;
-  uint32_t set_epoch = 1;
-  int64_t fast_reset_counter = 0;
+  uint32_t set_offset = 0;
+  int64_t fast_reset_counter = 0;  // calls since the last reset (the reference's is process-wide)
   uint32_t epoch = 0;                 // call id for touch marks
   uint32_t n_blocks = 0;              // pool slots in use (host copy, exact after a drain)
   uint32_t* d_nblocks = nullptr;      // [2] device copy, ping-pong: k_assign reads [nb_cur], writes [nb_cur ^ 1]
@@ -351,6 +357,7 @@ struct vbx_ctx {
   uint64_t counters[16] = {0};
   uint64_t apply_paths[16] = {0};  // ScanState::apply_paths of the last call whose status reached the host
   bool count_apply_paths = false;  // k_apply counts its paths (vbx_debug_count_apply_paths; vbx_debug_apply always does)
+  bool serial_fast = false;        // Fast calls walk their rays on one thread, in rank order (vbx_debug_serial_fast)
   uint64_t async_wait_ns = 0, async_submit_ns = 0;  // host time of vbx_tsdf_integrate_async: waiting for a hand-off set / enqueueing
   uint64_t esdf_counters[16] = {0};
   float last_ms = 0.f;
@@ -398,6 +405,7 @@ struct ScanRoute {
 };
 // The synchronous calls: hand-off set 0 and front lane 0 on the main stream, grids for the whole GPU.
 inline ScanRoute sync_route(vbx_ctx* c) { return {c->set[0], c->lane[0], c->stream, c->grid_sms, c->profiling}; }
+int init_fast_sets(vbx_ctx* c, cudaStream_t s);  // both sets cleared and word 0 marked, as a fresh ApproxHashSet
 int integrate_device(vbx_ctx* c, const ScanRoute& x, int kind, const float q[4], const float t[3], const float* d_xyz,
                      const uint8_t* d_rgba, uint64_t n, int freespace);
 
