@@ -15,6 +15,7 @@ import numpy as np  # noqa: E402
 
 from oracle import pyoracle as po  # noqa: E402
 from tests import test_block_sizes_gpu as tb  # noqa: E402
+from tests import test_esdf_fixed_point_gpu as tfp  # noqa: E402
 from tests import test_esdf_options_gpu as teo  # noqa: E402
 from tests import test_esdf_reference_gpu as te  # noqa: E402
 from tests import test_fast_reference_gpu as tf  # noqa: E402
@@ -41,6 +42,8 @@ def cases():
         out[f"esdf/{key}"] = lambda lib, k=key: te.reference_side(k, lib)[2]
     for key in teo.PIN_KEYS:
         out[f"esdf_options/{key}"] = lambda lib, k=key: teo.reference_side(k, lib)[2]
+    for key in tfp.PIN_KEYS:
+        out[f"esdf_fixed_point/{key}"] = lambda lib, k=key: tfp.reference_side(k, lib)[1]
     for key in tte.PIN_KEYS:
         out[f"tsdf_edges/{key}"] = lambda lib, k=key: tte.reference_side(k, lib)[3]
     for key in tg.PIN_KEYS:
