@@ -1,8 +1,8 @@
-"""-m gpu: the Merged ray trace runs in the front half against the hand-off set's private block table, and
-k_assign creates the blocks in submission order.  A table left dirty by an earlier scan of the same set, an id
-resolved twice across the passes of one call, or a fallback ray that bypasses the table would give wrong block
-ids: wrong voxels, or wrong touched / allocated counts.  Maps are compared bit for bit (distance, weight,
-colour, updated bits, block set) with synchronous calls and with the reference's own MergedTsdfIntegrator at one
+"""-m gpu: every integrator's ray walk runs in the front half against the hand-off set's private block table,
+and k_assign creates the blocks in submission order.  A table left dirty by an earlier scan of the same set, an
+id resolved twice across the passes of one call, or a fallback ray that bypasses the table would give wrong
+block ids: wrong voxels, or wrong touched / allocated counts.  Maps are compared bit for bit (distance, weight,
+colour, updated bits, block set) with synchronous calls and with the reference's own TsdfIntegrator at one
 thread (oracle/_ref) where that library exists, else with the restatement pinned to it; per-call counters with
 the restatement (the reference's harness does not count)."""
 import numpy as np
@@ -26,13 +26,13 @@ def _layer_bytes(layer):
     return idx.tobytes(), vox.tobytes(), np.asarray(upd).tobytes()
 
 
-def _reference_map(voxel):
+def _reference_map(voxel, **cfg):
     which = "reference" if po.available("reference") else "port"
-    return po.OracleMap(po.OracleLib(which), po.TsdfConfig(**CFG), voxel, 16)
+    return po.OracleMap(po.OracleLib(which), po.TsdfConfig(**CFG, **cfg), voxel, 16)
 
 
-def _port_map(voxel):
-    return po.OracleMap(po.OracleLib("port"), po.TsdfConfig(**CFG), voxel, 16)
+def _port_map(voxel, **cfg):
+    return po.OracleMap(po.OracleLib("port"), po.TsdfConfig(**CFG, **cfg), voxel, 16)
 
 
 def _assert_bit_exact(rep):
@@ -46,15 +46,15 @@ def _shifted(s, offset):
     return s[0], s[1], s[2], (np.asarray(s[3], np.float64) + offset).astype(np.float32)
 
 
-def test_pipelined_scans_alternating_between_disjoint_regions(monkeypatch):
+def _alternate_between_disjoint_regions(monkeypatch, kind):
     """Two hand-off sets, reused scan after scan, each seeing every region in turn: the private table of
     a set must be clean when its next scan starts, whatever blocks the previous one met."""
     monkeypatch.setenv("VBX_ASYNC_SETS", "2")
     opts = dict(max_updates_per_pass=1 << 22)
     la = vb.Layer(0.1, 16, engine_options=vb.EngineOptions(**opts))
     ls = vb.Layer(0.1, 16, engine_options=vb.EngineOptions(**opts))
-    ia = vb.TsdfIntegratorFactory.create("merged", vb.TsdfIntegratorConfig(**CFG), la)
-    isync = vb.TsdfIntegratorFactory.create("merged", vb.TsdfIntegratorConfig(**CFG), ls)
+    ia = vb.TsdfIntegratorFactory.create(kind, vb.TsdfIntegratorConfig(**CFG), la)
+    isync = vb.TsdfIntegratorFactory.create(kind, vb.TsdfIntegratorConfig(**CFG), ls)
     offsets = [np.zeros(3), np.array([25.0, 0.0, 0.0]), np.array([0.0, -30.0, 6.0])]
     rooms = scenes.c3_room_sequence(n_scans=21, width=160, height=120)
     scans = [_shifted(s, offsets[i % 3]) for i, s in enumerate(rooms)]
@@ -77,6 +77,14 @@ def test_pipelined_scans_alternating_between_disjoint_regions(monkeypatch):
     la.sync()
     assert _layer_bytes(la) == _layer_bytes(ls)
     assert ia.counters()["kernel_launches"] == isync.counters()["kernel_launches"] + 1
+
+
+def test_pipelined_scans_alternating_between_disjoint_regions(monkeypatch):
+    _alternate_between_disjoint_regions(monkeypatch, "merged")
+
+
+def test_pipelined_simple_scans_alternating_between_disjoint_regions(monkeypatch):
+    _alternate_between_disjoint_regions(monkeypatch, "simple")
 
 
 def _axis_scan():
@@ -121,21 +129,23 @@ def test_sequential_fallback_rays_use_the_scan_table():
     _assert_bit_exact(rep)
 
 
-def test_multi_pass_call_resolves_each_block_once():
+def _multi_pass_call(kind, extra):
     """The sensor's block (and its neighbours) receive records in every pass: one local id per block for
-    the whole call, so blocks_touched is the call's count, not a sum over passes."""
+    the whole call, so blocks_touched is the call's count, not a sum over passes.  Only the call's last pass
+    clears the table: a pass that cleared it early would draw a second id for a block met again."""
     scans = scenes.c3_room_sequence(n_scans=3, width=128, height=96)
-    cfg = vb.TsdfIntegratorConfig(**CFG)
+    cfg = vb.TsdfIntegratorConfig(**CFG, **extra)
     lp = vb.Layer(0.1, 16, engine_options=vb.EngineOptions(max_updates_per_pass=4096))
     l1 = vb.Layer(0.1, 16)
-    ip = vb.TsdfIntegratorFactory.create("merged", cfg, lp)
-    i1 = vb.TsdfIntegratorFactory.create("merged", cfg, l1)
-    ref, port = _reference_map(0.1), _port_map(0.1)
+    ip = vb.TsdfIntegratorFactory.create(kind, cfg, lp)
+    i1 = vb.TsdfIntegratorFactory.create(kind, cfg, l1)
+    ref, port = _reference_map(0.1, **extra), _port_map(0.1, **extra)
+    ref_kind = {"simple": po.SIMPLE, "merged": po.MERGED}[kind]
     for s in scans:
         ip.integratePointCloud((s[2], s[3]), s[0], s[1])
         i1.integratePointCloud((s[2], s[3]), s[0], s[1])
-        ref.integrate(2, s)
-        port.integrate(2, s)
+        ref.integrate(ref_kind, s)
+        port.integrate(ref_kind, s)
         gp, g1, oc = ip.counters(), i1.counters(), port.counters()
         assert gp["passes"] > 2, gp
         for k in ("rays", "clear_rays", "updates", "blocks_touched", "blocks_allocated"):  # (voxels: summed per pass)
@@ -152,3 +162,13 @@ def test_multi_pass_call_resolves_each_block_once():
     assert ip.counters()["passes"] == 1, ip.counters()
     assert ip.counters()["blocks_touched"] == i1.counters()["blocks_touched"]
     assert _layer_bytes(lp) == _layer_bytes(l1)
+
+
+def test_multi_pass_call_resolves_each_block_once():
+    _multi_pass_call("merged", {})
+
+
+@pytest.mark.parametrize("kind,extra", [pytest.param("simple", {}, id="simple"),
+                                        pytest.param("merged", dict(enable_anti_grazing=1), id="merged_anti_grazing")])
+def test_multi_pass_call_of_another_walk_resolves_each_block_once(kind, extra):
+    _multi_pass_call(kind, extra)

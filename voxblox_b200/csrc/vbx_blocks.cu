@@ -72,7 +72,6 @@ int rebuild_hash(vbx_ctx* c) {
   cudaStream_t s = c->stream;
   VBX_CUDA(c, cudaMemsetAsync(c->tab.hkeys, 0xff, (size_t)c->hcap * sizeof(uint64_t), s));
   VBX_CUDA(c, cudaMemsetAsync(c->tab.hslot, 0xff, (size_t)c->hcap * sizeof(int32_t), s));
-  VBX_CUDA(c, cudaMemsetAsync(c->tab.htouch, 0, (size_t)c->hcap * sizeof(unsigned long long), s));
   if (c->n_blocks) k_rebuild_hash<<<grid_for(c->n_blocks, 256), 256, 0, s>>>(c->tab, c->n_blocks);
   VBX_CUDA(c, cudaStreamSynchronize(s));
   VBX_CUDA(c, cudaGetLastError());
@@ -270,7 +269,6 @@ int clear_layer(vbx_ctx* c, int layer) {
   VBX_CUDA(c, cudaMemsetAsync(c->tab.tsdf, 0, used * sizeof(TsdfVoxel), s));
   VBX_CUDA(c, cudaMemsetAsync(c->tab.hkeys, 0xff, (size_t)c->hcap * sizeof(uint64_t), s));
   VBX_CUDA(c, cudaMemsetAsync(c->tab.hslot, 0xff, (size_t)c->hcap * sizeof(int32_t), s));
-  VBX_CUDA(c, cudaMemsetAsync(c->tab.htouch, 0, (size_t)c->hcap * sizeof(unsigned long long), s));
   VBX_CUDA(c, cudaMemsetAsync(c->tab.slot_updated, 0, c->tab.max_blocks, s));
   VBX_CUDA(c, cudaMemsetAsync(c->tab.slot_esdf_updated, 0, c->tab.max_blocks, s));
   VBX_CUDA(c, cudaMemsetAsync(c->tab.slot_has_esdf, 0, c->tab.max_blocks, s));

@@ -352,9 +352,9 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
   t.max_blocks = o.max_blocks;
   CK(dmalloc(&t.hkeys, hcap));
   CK(dmalloc(&t.hslot, hcap));
-  CK(dmalloc(&t.htouch, hcap));
   CK(dmalloc(&t.new_list, o.max_blocks));
-  // ids lost to first-touch races stay unused (vbx_hash.cuh); (id, voxel) must fit a 32-bit record key
+  // one local id per block a call touches (vbx_hash.cuh, scan_block_id), with headroom past the pool;
+  // (id, voxel) must fit a 32-bit record key
   t.touched_cap = (uint32_t)std::min<uint64_t>((uint64_t)o.max_blocks + 65536u, (0xffffffffull >> (3 * c->L)) - 1);
   t.vox_per_block = c->vox_per_block;
   CK(dmalloc(&t.slot_key, o.max_blocks));
@@ -364,7 +364,6 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
   CK(dmalloc(&t.tsdf, (size_t)o.max_blocks * c->vox_per_block));
   CK(cudaMemsetAsync(t.hkeys, 0xff, (size_t)hcap * sizeof(uint64_t), c->stream));
   CK(cudaMemsetAsync(t.hslot, 0xff, (size_t)hcap * sizeof(int32_t), c->stream));
-  CK(cudaMemsetAsync(t.htouch, 0, (size_t)hcap * sizeof(unsigned long long), c->stream));
   CK(cudaMemsetAsync(t.slot_updated, 0, o.max_blocks, c->stream));
   CK(cudaMemsetAsync(t.slot_esdf_updated, 0, o.max_blocks, c->stream));
   CK(cudaMemsetAsync(t.slot_has_esdf, 0, o.max_blocks, c->stream));
@@ -460,7 +459,7 @@ void vbx_destroy(vbx_ctx* c) {
   mesh_destroy(c);
   icp_destroy(c);
   Tables& t = c->tab;
-  void* ptrs[] = {t.hkeys,    t.hslot,        t.htouch,       t.new_list,   t.slot_key,     t.slot_updated,
+  void* ptrs[] = {t.hkeys,    t.hslot,        t.new_list,   t.slot_key,     t.slot_updated,
                   t.slot_esdf_updated, t.slot_has_esdf, t.tsdf, c->order, c->order_inv, c->set_start,
                   c->set_observed, c->d_nblocks, c->d_hold};
   for (void* p : ptrs) {

@@ -116,7 +116,7 @@ struct ScanState {
   uint32_t esdf_ticket[6];   // ESDF queue kernels: work hand-out counters, rotating like the queue counters ([0..2] raise, [3..5] lower)
   uint32_t tile_ticket;      // k_apply: record tiles of the short runs handed out
   uint32_t apply_paths[12];  // k_apply: how often each arithmetic path ran, summed over the call (ApplyPath)
-  uint32_t ids_resolved;     // Merged: local block ids k_assign has resolved so far in this call (all passes)
+  uint32_t ids_resolved;     // local block ids k_assign has resolved so far in this call (all passes)
   uint32_t reserved;
 };
 static_assert(sizeof(ScanState) == 256, "the status block the host reads back is 256 bytes");
@@ -127,7 +127,6 @@ static_assert(sizeof(ScanState::apply_paths) / 4 == kApplyPaths, "one word per a
 struct Tables {
   uint64_t* hkeys;        // [hcap] packed block index, kEmptyKey when free
   int32_t* hslot;         // [hcap] pool slot
-  unsigned long long* htouch;  // [hcap] (call id << 32 | touched id) of the last call that touched the block
   uint32_t hmask;         // hcap - 1
   uint32_t max_blocks;
   uint32_t vox_per_block;
@@ -142,10 +141,10 @@ struct Tables {
   EsdfVoxel* esdf;        // [max_blocks << 3L] (allocated by vbx_esdf_create)
 };
 
-// A Merged scan's private block table (hand-off set private, beside touched_list).  The ray trace runs in
-// the front half, beside other scans' map-touching stages, so it must not read the block hash: it gives the
-// blocks it meets dense local ids here instead, and k_assign (walk stage, submission order) resolves each
-// id against the hash.  Open addressing keyed by pack3(block), value = local id + 1 (0: free).  The table is
+// A scan's private block table (hand-off set private, beside touched_list).  The ray walk that writes the
+// update records runs in the front half, beside other scans' map-touching stages, so it must not read the
+// block hash: it gives the blocks it meets dense local ids here instead, and k_assign (walk stage, submission
+// order) resolves each id against the hash, creating the blocks that are missing.  Open addressing keyed by pack3(block), value = local id + 1 (0: free).  The table is
 // zeroed once when it is allocated; k_assign clears the positions a call used.
 struct ScanBlocks {
   uint32_t* table;            // [mask + 1], a power of two >= 2 * cap
@@ -212,12 +211,12 @@ struct vbx_ctx {
   unsigned long long* set_observed = nullptr;
   uint32_t set_offset = 0;
   int64_t fast_reset_counter = 0;  // calls since the last reset (the reference's is process-wide)
-  uint32_t epoch = 0;                 // call id for touch marks
   uint32_t n_blocks = 0;              // pool slots in use (host copy, exact after a drain)
   uint32_t* d_nblocks = nullptr;      // [2] device copy, ping-pong: k_assign reads [nb_cur], writes [nb_cur ^ 1]
   int nb_cur = 0;
   // Asynchronous submission (vbx_tsdf_integrate_async): a scan passes through four stages -- front half
-  // (keys, bundle sort, bundle fold, offsets, Merged's ray trace; does not touch the map) on one of kLanes
+  // (keys, bundle sort, bundle fold, offsets, the ray walk that writes the update records; does not touch
+  // the map) on one of kLanes
   // front lanes, block creation, record sort, apply -- so up to kSets scans are in flight, each owning one set
   // of hand-off buffers.  Map-touching stages run in submission order.  Each scan is one launch of a CUDA
   // graph per (hand-off set, front lane, kind), captured before its first use.  The sets and lanes are the
@@ -244,8 +243,8 @@ struct vbx_ctx {
     uint2* ray_c = nullptr;          // [max_points] colour, weight bits
     uint32_t* ray_list = nullptr;    // [max_points] Merged: ray slot (rank in the reference's bundle order) -> head
     uint32_t* head_list = nullptr;   // bundle id -> sorted position of its head (read again by the ray walk)
-    uint32_t* touched_list = nullptr;  // touched id -> hash position (written by k_assign / the walk, read by the apply)
-    vbx::ScanBlocks blocks{};          // Merged: local block ids of the trace (written by the front half, read by k_assign)
+    uint32_t* touched_list = nullptr;  // touched id -> hash position (written by k_assign, read by the apply)
+    vbx::ScanBlocks blocks{};          // local block ids of the ray walk (written by the front half, read by k_assign)
     uint32_t* cnt = nullptr;         // [max_points + 1]
     uint32_t* off = nullptr;         // [max_points + 1]
     vbx::ScanState* d_state = nullptr;
@@ -298,7 +297,7 @@ struct vbx_ctx {
   bool async_ready = false;
   int prio_lo = 0, prio_hi = 0;  // stream priority range of the device
   // the streams a scan's graph is captured from (besides the front lane's and the main stream)
-  cudaStream_t stream_e = nullptr;  // block creation: k_back_begin, k_assign (Simple: and its ray walk)
+  cudaStream_t stream_e = nullptr;  // block creation: k_back_begin, k_assign
   cudaStream_t stream_s = nullptr;  // record sort + apply preparation
   cudaEvent_t cap_ev[8] = {};  // capture-internal edges (fork, front -> walk, walk -> sort, sort -> apply, joins)
   uint64_t async_seq = 0;

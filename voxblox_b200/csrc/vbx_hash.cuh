@@ -63,53 +63,20 @@ __device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
   return v;
 }
 
-__device__ __forceinline__ unsigned long long ld_acquire_gpu(const unsigned long long* p) {
-  unsigned long long v;
-  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
-
-// An id word that a thread has claimed and not yet filled in: the thread that wins a block draws its id
-// only after its claim succeeded, so a race for a block's first touch draws ONE id, however many threads
+// ------------------------------------------------------ scan-private block table
+// A table position that a thread has claimed and not yet filled in: the thread that wins a block draws its
+// id only after its claim succeeded, so a race for a block's first touch draws ONE id, however many threads
 // take part.  (At voxels_per_side 1 every walk step is a new block and thousands of rays leave the sensor
-// together: drawing before the claim burnt an id per racing thread, ~100x the blocks a scan touches.)
+// together: drawing before the claim would burn an id per racing thread, ~100x the blocks a scan touches.)
 constexpr uint32_t kPendingId = 0xffffffffu;
 
-// Blocks touched by the current call get dense ids 0, 1, 2, ... (update records are keyed by
-// (touched id, voxel in block): a handful of bits instead of a hash position).  The per-position
-// word packs (call id, touched id); the first toucher of a block in this call claims the word with
-// one CAS (call id, kPendingId), draws the id and publishes it; the others wait for it.  Only this
-// call's walk writes these words, so n_touch_ids == n_touched.
-__device__ __forceinline__ uint32_t touch_block(const Tables& t, uint32_t hp, uint32_t epoch, ScanState* st) {
-  unsigned long long* w = t.htouch + hp;
-  const unsigned long long mine = (unsigned long long)epoch << 32;
-  unsigned long long cur = ld_acquire_gpu(w);
-  while ((uint32_t)(cur >> 32) != epoch) {
-    const unsigned long long old = atomicCAS(w, cur, mine | kPendingId);
-    if (old == cur) {
-      uint32_t id = atomicAdd(&st->n_touch_ids, 1u);
-      if (id < t.touched_cap) {
-        t.touched_list[id] = hp;
-        atomicAdd(&st->n_touched, 1u);
-      } else {
-        atomicOr(&st->error, kErrPoolFull);
-        id = 0u;  // (the call fails; the waiting threads must not spin on the claim)
-      }
-      atomicExch(w, mine | id);
-      return id;
-    }
-    cur = old;
-  }
-  while ((uint32_t)cur == kPendingId) cur = ld_acquire_gpu(w);  // another thread of this call claimed the block
-  return (uint32_t)cur;
-}
-
-// ------------------------------------------------------ scan-private block table
-// The local id of a block in the scan's private table (ScanBlocks), drawn from the same counter, without
-// reading the block hash.  The first thread to meet a free position claims it with one CAS (kPendingId),
-// draws an id, lists its key and position under it and then publishes id + 1 at the position.  A reader that
-// meets a claimed position waits for the id, then compares the key listed under it.  Every id drawn names a
-// block (ids drawn past the capacity raise kErrPoolFull and free the position again).
+// The local id of a block in the scan's private table (ScanBlocks), drawn from ScanState::n_touch_ids, without
+// reading the block hash: blocks touched by the call get dense ids 0, 1, 2, ... (update records are keyed by
+// (local id, voxel in block): a handful of bits instead of a hash position).  The first thread to meet a free
+// position claims it with one CAS (kPendingId), draws an id, lists its key and position under it and then
+// publishes id + 1 at the position.  A reader that meets a claimed position waits for the id, then compares
+// the key listed under it.  Every id drawn names a block (ids drawn past the capacity raise kErrPoolFull and
+// free the position again).
 __device__ inline uint32_t scan_block_id(const ScanBlocks& b, uint64_t key, ScanState* st) {
   uint32_t pos = hash64(key) & b.mask;
   for (uint32_t probe = 0; probe <= b.mask;) {
