@@ -1,8 +1,9 @@
 """Generates tests/golden/reference_pins.json (see reference_pins.py) from the reference's own library,
 oracle/_ref/libvbx_ref.so.  Run it where that library was built; it needs no GPU:
 
-    python tests/golden/make_reference_pins.py
+    python tests/golden/make_reference_pins.py [key prefix ...]
 
+With key prefixes, only the keys that start with one of them are recomputed; the others are kept as recorded.
 It also runs the restatement on every case and reports where the two differ."""
 import json
 import os
@@ -15,6 +16,7 @@ import numpy as np  # noqa: E402
 
 from oracle import pyoracle as po  # noqa: E402
 from tests import test_block_sizes_gpu as tb  # noqa: E402
+from tests import test_esdf_fe_gpu as tfe  # noqa: E402
 from tests import test_esdf_fixed_point_gpu as tfp  # noqa: E402
 from tests import test_esdf_options_gpu as teo  # noqa: E402
 from tests import test_esdf_reference_gpu as te  # noqa: E402
@@ -44,6 +46,11 @@ def cases():
         out[f"esdf_options/{key}"] = lambda lib, k=key: teo.reference_side(k, lib)[2]
     for key in tfp.PIN_KEYS:
         out[f"esdf_fixed_point/{key}"] = lambda lib, k=key: tfp.reference_side(k, lib)[1]
+    for key in tfe.PIN_KEYS:
+        if key.startswith("synthetic/"):
+            out[f"esdf_fe/{key}"] = lambda lib, k=key: tfe.synthetic_reference_side(k.split("/", 1)[1], lib)[1]
+        else:
+            out[f"esdf_fe/{key}"] = lambda lib, k=key: tfe.reference_side(k, lib)[1]
     for key in tte.PIN_KEYS:
         out[f"tsdf_edges/{key}"] = lambda lib, k=key: tte.reference_side(k, lib)[3]
     for key in tg.PIN_KEYS:
@@ -60,10 +67,12 @@ def cases():
     return out
 
 
-def main():
+def main(prefixes=()):
     ref, port = po.OracleLib("reference"), po.OracleLib("port")
-    pinned = {}
+    pinned = json.load(open(pins.PATH)) if prefixes else {}
     for key, fn in cases().items():
+        if prefixes and not key.startswith(tuple(prefixes)):
+            continue
         pinned[key] = fn(ref)
         if key.startswith("icp/refine") or key.startswith("block_sizes/icp/"):
             same = fn(port)["map"] == pinned[key]["map"]   # the restatement's ICP is compared at 1e-5, not bit for bit
@@ -79,4 +88,4 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1:])
