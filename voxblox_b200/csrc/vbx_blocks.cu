@@ -13,34 +13,21 @@
 
 namespace vbx {
 
-__global__ void k_ensure_keys(Tables tab, const uint64_t* __restrict__ keys, uint32_t m, uint32_t* __restrict__ hp_out,
-                              ScanState* st) {
+// an uploaded block's local id in the hand-off set's table (k_assign creates the missing blocks)
+__global__ void k_list_keys(ScanBlocks sb, const uint64_t* __restrict__ keys, uint32_t m, uint32_t* __restrict__ ids,
+                            ScanState* st) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= m) return;
-  hp_out[i] = ensure_block(tab, keys[i], st);
+  ids[i] = scan_block_id(sb, keys[i], st);
 }
 
-__global__ void k_assign_uploaded(Tables tab, uint32_t n_blocks_before, uint8_t new_slot_flags, ScanState* st) {
-  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t n_new = min(st->n_new, tab.max_blocks);
-  if (j < n_new) {
-    const uint32_t slot = n_blocks_before + j;
-    if (slot < tab.max_blocks) {
-      const uint32_t hp = tab.new_list[j];
-      tab.hslot[hp] = (int32_t)slot;
-      tab.slot_key[slot] = tab.hkeys[hp];
-      tab.slot_updated[slot] = new_slot_flags;
-    } else {
-      atomicOr(&st->error, kErrPoolFull);
-    }
-  }
-  if (j == 0) st->n_blocks = min(n_blocks_before + st->n_new, tab.max_blocks);
-}
-
-__global__ void k_slots_of(Tables tab, const uint32_t* __restrict__ hp, uint32_t m, int32_t* __restrict__ slot_out) {
+// ... and its pool slot once k_assign has resolved the id to a hash position (touched_list)
+__global__ void k_slots_of(const int32_t* __restrict__ hslot, const uint32_t* __restrict__ touched_list,
+                           const uint32_t* __restrict__ ids, uint32_t m, int32_t* __restrict__ slot_out) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= m) return;
-  slot_out[i] = hp[i] == 0xffffffffu ? -1 : tab.hslot[hp[i]];
+  const uint32_t hp = ids[i] == 0xffffffffu ? 0xffffffffu : touched_list[ids[i]];
+  slot_out[i] = hp == 0xffffffffu ? -1 : hslot[hp];
 }
 
 // rebuild the hash from the per-slot keys (after blocks were removed and the pool compacted)
@@ -199,30 +186,41 @@ int upload_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, const 
     }
     keys[i] = pack3(p[0], p[1], p[2]);
   }
-  // scratch of hand-off set 0: the point-key buffer holds the keys, the ray list the hash positions, cnt the slots
+  // scratch of hand-off set 0: the point-key buffer holds the keys, the ray list their local ids, cnt the slots
   if (m > c->max_points) return fail(c, VBX_E_CAPACITY, "upload more than max_points_per_scan blocks at once");
   const vbx_ctx::ScratchSet& S = c->set[0];
   VBX_CUDA(c, cudaMemcpyAsync(S.pkeys0, keys.data(), m * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
-  VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), s));
-  k_ensure_keys<<<grid_for(m, 256), 256, 0, s>>>(c->tab, S.pkeys0, (uint32_t)m, S.ray_list, S.d_state);
-  // a block inserted into the ESDF layer at an index the TSDF layer does not hold occupies a slot of its own
-  k_assign_uploaded<<<grid_for(c->tab.max_blocks, 256), 256, 0, s>>>(
-      c->tab, c->n_blocks, layer == VBX_LAYER_ESDF ? kSlotNoTsdf : (uint8_t)0, S.d_state);
-  k_slots_of<<<grid_for(m, 256), 256, 0, s>>>(c->tab, S.ray_list, (uint32_t)m, reinterpret_cast<int32_t*>(S.cnt));
-  VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
-  VBX_CUDA(c, cudaStreamSynchronize(s));
-  if (S.h_state->error & kFatalErrors) return fail(c, VBX_E_CAPACITY, "block pool / hash full during upload");
-  if (layer == VBX_LAYER_ESDF && S.h_state->n_new) c->maybe_esdf_only = true;
-  if (int rc = set_n_blocks(c, S.h_state->n_blocks)) return rc;
+  // every block is created by k_assign, in rounds of at most as many keys as the table has ids; a block
+  // inserted into the ESDF layer at an index the TSDF layer does not hold occupies a slot of its own
+  const uint8_t new_bits = layer == VBX_LAYER_ESDF ? kSlotNoTsdf : (uint8_t)0;
+  int err = VBX_OK;
+  uint64_t listed = 0;  // keys whose slots are known (a round that fails ends the listing)
+  while (listed < m && err == VBX_OK) {
+    const uint32_t rn = (uint32_t)std::min<uint64_t>(S.blocks.cap, m - listed);
+    VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), s));
+    k_list_keys<<<grid_for(rn, 256), 256, 0, s>>>(S.blocks, S.pkeys0 + listed, rn, S.ray_list + listed, S.d_state);
+    if (int rc = create_listed_blocks(c, new_bits)) return rc;
+    k_slots_of<<<grid_for(rn, 256), 256, 0, s>>>(c->tab.hslot, S.touched_list, S.ray_list + listed, rn,
+                                                  reinterpret_cast<int32_t*>(S.cnt) + listed);
+    VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+    VBX_CUDA(c, cudaStreamSynchronize(s));
+    const ScanState& h = *S.h_state;
+    c->n_blocks = h.n_blocks;
+    if (layer == VBX_LAYER_ESDF && h.n_new) c->maybe_esdf_only = true;
+    err = check_state_errors(c, h);
+    listed += rn;
+  }
+  // The payloads of the blocks that have slots, also when the pool ran out: every block the call created
+  // holds what was uploaded for it (an ESDF block becomes one only here, by slot_has_esdf)
   const size_t bbytes = payload_bytes(c, layer, serialized);
   const uint32_t wpv = (layer == VBX_LAYER_TSDF) ? 3u : (serialized ? 1u : 5u);  // threads per voxel along x
   uint32_t* pool = layer == VBX_LAYER_TSDF ? reinterpret_cast<uint32_t*>(c->tab.tsdf) : reinterpret_cast<uint32_t*>(c->tab.esdf);
   uint8_t* flags = layer == VBX_LAYER_TSDF ? c->tab.slot_updated : c->tab.slot_esdf_updated;
-  const uint64_t chunk = std::max<uint64_t>(1, std::min<uint64_t>(m, (256ull << 20) / bbytes));
+  const uint64_t chunk = std::max<uint64_t>(1, std::min<uint64_t>(listed, (256ull << 20) / bbytes));
   if (int rc = ensure_staging(c, chunk * bbytes + chunk, chunk)) return rc;
   uint8_t* d_upd = static_cast<uint8_t*>(c->mirror_dev) + chunk * bbytes;
-  for (uint64_t at = 0; at < m; at += chunk) {
-    const uint64_t k = std::min<uint64_t>(chunk, m - at);
+  for (uint64_t at = 0; at < listed; at += chunk) {
+    const uint64_t k = std::min<uint64_t>(chunk, listed - at);
     VBX_CUDA(c, cudaMemcpyAsync(c->mirror_dev, static_cast<const char*>(voxels) + at * bbytes, k * bbytes,
                                 cudaMemcpyHostToDevice, s));
     if (updated_bits) VBX_CUDA(c, cudaMemcpyAsync(d_upd, updated_bits + at, k, cudaMemcpyHostToDevice, s));
@@ -237,6 +235,7 @@ int upload_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, const 
     }
     VBX_CUDA(c, cudaStreamSynchronize(s));  // the staging buffer is reused by the next chunk
   }
+  if (err) return err;
   return refresh_host_mirror(c);
 }
 

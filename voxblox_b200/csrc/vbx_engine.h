@@ -144,8 +144,10 @@ struct Tables {
 // A scan's private block table (hand-off set private, beside touched_list).  The ray walk that writes the
 // update records runs in the front half, beside other scans' map-touching stages, so it must not read the
 // block hash: it gives the blocks it meets dense local ids here instead, and k_assign (walk stage, submission
-// order) resolves each id against the hash, creating the blocks that are missing.  Open addressing keyed by pack3(block), value = local id + 1 (0: free).  The table is
-// zeroed once when it is allocated; k_assign clears the positions a call used.
+// order) resolves each id against the hash, creating the blocks that are missing.  Uploads and robot-position
+// spheres list their blocks in hand-off set 0's table the same way.  Open addressing keyed by pack3(block),
+// value = local id + 1 (0: free).  The table is zeroed once when it is allocated; k_assign clears the
+// positions a call used.
 struct ScanBlocks {
   uint32_t* table;            // [mask + 1], a power of two >= 2 * cap
   unsigned long long* keys;   // [cap] local id -> packed block index
@@ -405,6 +407,13 @@ struct ScanRoute {
 // The synchronous calls: hand-off set 0 and front lane 0 on the main stream, grids for the whole GPU.
 inline ScanRoute sync_route(vbx_ctx* c) { return {c->set[0], c->lane[0], c->stream, c->grid_sms, c->profiling}; }
 int init_fast_sets(vbx_ctx* c, cudaStream_t s);  // both sets cleared and word 0 marked, as a fresh ApproxHashSet
+// The blocks an upload or a robot-position sphere listed in hand-off set 0's table (scan_block_id), created by
+// k_assign as a scan's are, on the main stream: blocks that exist keep their updated bits, a new slot's start
+// at new_bits, and the block count moves as after a scan.
+int create_listed_blocks(vbx_ctx* c, uint8_t new_bits);
+// A finished call's status block: VBX_E_CAPACITY for a device error; a full pool also takes h.n_blocks and
+// rebuilds the hash (the call's surplus entries have no slot)
+int check_state_errors(vbx_ctx* c, const ScanState& h);
 int integrate_device(vbx_ctx* c, const ScanRoute& x, int kind, const float q[4], const float t[3], const float* d_xyz,
                      const uint8_t* d_rgba, uint64_t n, int freespace);
 

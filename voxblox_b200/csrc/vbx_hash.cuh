@@ -32,20 +32,6 @@ __device__ inline uint32_t find_or_insert_block(const Tables& t, uint64_t key, b
   return 0xffffffffu;
 }
 
-__device__ inline uint32_t ensure_block(const Tables& t, uint64_t key, ScanState* st) {
-  bool created;
-  const uint32_t hp = find_or_insert_block(t, key, &created, st);
-  if (created) {
-    const uint32_t j = atomicAdd(&st->n_new, 1u);
-    if (j < t.max_blocks) {
-      t.new_list[j] = hp;
-    } else {
-      atomicOr(&st->error, kErrPoolFull);
-    }
-  }
-  return hp;
-}
-
 __device__ __forceinline__ uint32_t find_block(const Tables& t, uint64_t key) {
   uint32_t hp = hash64(key) & t.hmask;
   for (uint32_t probe = 0; probe <= t.hmask; ++probe) {

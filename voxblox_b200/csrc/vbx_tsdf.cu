@@ -1235,16 +1235,18 @@ __global__ void k_back_begin(ScanState* st, uint32_t* hold) {
   }
 }
 
-// The walk stage's own work, in submission order: one thread block.  The ray walk (front half) gave every
-// block it met a local id in the scan's private table; here each id listed since the last pass finds or
-// creates its block in the hash (allocateStorageAndGetVoxelPtr's find-or-emplace, cc:109-124), becomes the
-// touched id the apply resolves, and marks an existing block updated (cc:128).  The call's last pass clears
-// the table.  Then pool slots for the blocks created by this call (updateLayerWithStoredBlocks,
-// cc:137-147); a new block is born with all updated bits set (cc:128).
+// The walk stage's own work, in submission order: one thread block, and the only place blocks are created.
+// The ray walk (front half), an upload or a robot-position sphere gave every block it met a local id in the
+// hand-off set's private table; here each id listed since the last pass finds or creates its block in the
+// hash (allocateStorageAndGetVoxelPtr's find-or-emplace, cc:109-124), becomes the touched id the apply
+// resolves, and an existing block's slot_updated becomes touch_bits (cc:128; 0 leaves it alone).  The call's
+// last pass clears the table.  Then pool slots for the blocks created by this call
+// (updateLayerWithStoredBlocks, cc:137-147), whose slot_updated starts at new_bits: a scan's new block is born
+// with all updated bits set (cc:128).
 constexpr int kAssignThreads = 512;
 __global__ void __launch_bounds__(kAssignThreads)
 k_assign(Tables tab, ScanBlocks sb, const ScanArgs* __restrict__ A, uint32_t* __restrict__ nb, SortPlan* record_plan,
-         ScanState* st) {
+         ScanState* st, uint8_t touch_bits, uint8_t new_bits) {
   const uint32_t* __restrict__ nb_in = nb + A->nb_cur;
   uint32_t* __restrict__ nb_out = nb + (A->nb_cur ^ 1u);
   const uint32_t t = threadIdx.x;
@@ -1273,7 +1275,7 @@ k_assign(Tables tab, ScanBlocks sb, const ScanArgs* __restrict__ A, uint32_t* __
         tab.touched_list[id] = hp;
         if (hp != 0xffffffffu) {
           const int32_t slot = tab.hslot[hp];
-          if (slot >= 0) tab.slot_updated[slot] = kTouchedBits;  // (*last_block)->updated().set(), cc:128
+          if (slot >= 0 && touch_bits) tab.slot_updated[slot] = touch_bits;  // (*last_block)->updated().set(), cc:128
           ++touched;
         }
       }
@@ -1312,7 +1314,7 @@ k_assign(Tables tab, ScanBlocks sb, const ScanArgs* __restrict__ A, uint32_t* __
       const uint32_t hp = tab.new_list[j];
       tab.hslot[hp] = (int32_t)slot;
       tab.slot_key[slot] = tab.hkeys[hp];
-      tab.slot_updated[slot] = kTouchedBits;
+      tab.slot_updated[slot] = new_bits;
     } else {
       atomicOr(&st->error, kErrPoolFull);
     }
@@ -2106,7 +2108,7 @@ int init_bundle_order(vbx_ctx* c) {
 
 static inline unsigned int grid_for(uint64_t n, int block) { return (unsigned int)((n + block - 1) / block); }
 
-static int check_state_errors(vbx_ctx* c, const ScanState& h) {
+int check_state_errors(vbx_ctx* c, const ScanState& h) {
   const uint32_t err = h.error & kFatalErrors;
   if (!err) return VBX_OK;
   if (err & kErrPoolFull) {
@@ -2383,14 +2385,19 @@ static int sort_and_apply(vbx_ctx* c, const ScanRoute& x, Tally& tally, const Ca
   return VBX_OK;
 }
 
+// k_assign on x.s for the blocks listed in the hand-off set's table; the block count moves to the other word
+// of d_nblocks.
+static void assign_blocks(vbx_ctx* c, const ScanRoute& x, uint8_t touch_bits, uint8_t new_bits) {
+  const vbx_ctx::ScratchSet& S = x.S;
+  k_assign<<<1, kAssignThreads, 0, x.s>>>(scan_tables(c, S), S.blocks, S.d_args, c->d_nblocks, S.sort_plan1,
+                                          S.d_state, touch_bits, new_bits);
+  c->nb_cur ^= 1;
+}
+
 // Block creation (k_assign, in submission order), then the record sort and the apply.
 static int back_half(vbx_ctx* c, const ScanRoute& x, Tally& tally, const Capture* cap = nullptr) {
-  cudaStream_t s = x.s;
-  const vbx_ctx::ScratchSet& S = x.S;
-  const Tables tab = scan_tables(c, S);
-  k_assign<<<1, kAssignThreads, 0, s>>>(tab, S.blocks, S.d_args, c->d_nblocks, S.sort_plan1, S.d_state);
+  assign_blocks(c, x, kTouchedBits, kTouchedBits);
   ++tally.launches;
-  c->nb_cur ^= 1;
   tally.mark(kStageAssign);
   return sort_and_apply(c, x, tally, cap);
 }
@@ -2410,6 +2417,17 @@ static void fill_args(const vbx_ctx* c, const ScanParams& P, const float* xyz, c
 static int upload_args(vbx_ctx* c, const ScanRoute& x, const ScanArgs& a) {
   *x.S.h_args = a;
   VBX_CUDA(c, cudaMemcpyAsync(x.S.d_args, x.S.h_args, sizeof(ScanArgs), cudaMemcpyHostToDevice, x.s));
+  return VBX_OK;
+}
+
+int create_listed_blocks(vbx_ctx* c, uint8_t new_bits) {
+  const ScanRoute x = sync_route(c);
+  ScanArgs a;
+  std::memset(&a, 0, sizeof(a));
+  a.P.emit_hi = 0xffffffffu;  // (>= P.n: k_assign clears the table, as a scan's last pass does)
+  a.nb_cur = (uint32_t)c->nb_cur;
+  if (int rc = upload_args(c, x, a)) return rc;
+  assign_blocks(c, x, 0, new_bits);
   return VBX_OK;
 }
 
