@@ -698,26 +698,6 @@ int vbx_sync(vbx_ctx* c) {
   return VBX_OK;
 }
 
-// Per-slot flag bytes of a layer with the engine's internal bits resolved: `has` = the layer holds a
-// block in this slot, `upd` = Block::updated() bits only.
-static int fetch_flags(vbx_ctx* c, int layer, std::vector<uint8_t>* upd, std::vector<uint8_t>* has) {
-  upd->resize(c->n_blocks);
-  has->assign(c->n_blocks, 1);
-  if (c->n_blocks == 0) return VBX_OK;
-  const uint8_t* src = (layer == VBX_LAYER_TSDF) ? c->tab.slot_updated : c->tab.slot_esdf_updated;
-  VBX_CUDA(c, cudaMemcpyAsync(upd->data(), src, c->n_blocks, cudaMemcpyDeviceToHost, c->stream));
-  if (layer == VBX_LAYER_ESDF) {
-    VBX_CUDA(c, cudaMemcpyAsync(has->data(), c->tab.slot_has_esdf, c->n_blocks, cudaMemcpyDeviceToHost,
-                                c->stream));
-  }
-  VBX_CUDA(c, cudaStreamSynchronize(c->stream));
-  for (uint32_t s = 0; s < c->n_blocks; ++s) {
-    if (layer == VBX_LAYER_TSDF && ((*upd)[s] & kSlotNoTsdf)) (*has)[s] = 0;
-    (*upd)[s] &= 0x07;  // kSlotNoTsdf / kEsdfPending / the mirror mark are internal
-  }
-  return VBX_OK;
-}
-
 int vbx_num_blocks(vbx_ctx* c, int layer, uint64_t* n) {
   if (!c || !n) return VBX_E_INVALID;
   VBX_CUDA(c, cudaSetDevice(c->device));
@@ -726,15 +706,9 @@ int vbx_num_blocks(vbx_ctx* c, int layer, uint64_t* n) {
     *n = c->n_blocks;
     return VBX_OK;
   }
-  if (layer == VBX_LAYER_ESDF && !c->has_esdf) {
-    *n = 0;
-    return VBX_OK;
-  }
-  std::vector<uint8_t> upd, has;
-  if (int rc = fetch_flags(c, layer, &upd, &has)) return rc;
-  uint64_t k = 0;
-  for (uint8_t h : has) k += h ? 1 : 0;
-  *n = k;
+  LayerSlots view;  // (no members in the ESDF layer before vbx_esdf_create)
+  if (int rc = read_layer_slots(c, layer, &view)) return rc;
+  *n = (uint64_t)std::count(view.member.begin(), view.member.end(), 1);
   return VBX_OK;
 }
 
@@ -743,27 +717,10 @@ int vbx_list_blocks(vbx_ctx* c, int layer, int updated_mask, int32_t* idx3, uint
   VBX_CUDA(c, cudaSetDevice(c->device));
   VBX_DRAIN(c);
   *n = 0;
-  if (layer == VBX_LAYER_ESDF && !c->has_esdf) return VBX_OK;
-  if (int rc = refresh_host_mirror(c)) return rc;
-  std::vector<uint8_t> upd, has;
-  if (int rc = fetch_flags(c, layer, &upd, &has)) return rc;
-  struct K3 {
-    int x, y, z;
-  };
-  std::vector<K3> keys;
-  keys.reserve(c->n_blocks);
-  for (uint32_t s = 0; s < c->n_blocks; ++s) {
-    if (!has[s]) continue;
-    if (updated_mask && !(upd[s] & updated_mask)) continue;
-    K3 k;
-    unpack3(c->host_slot_key[s], &k.x, &k.y, &k.z);
-    keys.push_back(k);
-  }
-  std::sort(keys.begin(), keys.end(), [](const K3& a, const K3& b) {
-    if (a.x != b.x) return a.x < b.x;
-    if (a.y != b.y) return a.y < b.y;
-    return a.z < b.z;
-  });
+  LayerSlots view;
+  if (int rc = read_layer_slots(c, layer, &view)) return rc;
+  // selected on the reported bits only: VBX_UPDATED_MIRROR lists nothing here
+  const std::vector<LayerSlots::Entry> keys = view.sorted(kReportedBits, updated_mask);
   *n = keys.size();
   if (idx3) {
     const uint64_t m = std::min<uint64_t>(cap, keys.size());
@@ -782,19 +739,20 @@ int vbx_download_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, 
   VBX_CUDA(c, cudaSetDevice(c->device));
   VBX_DRAIN(c);
   if (layer == VBX_LAYER_ESDF && !c->has_esdf) return fail(c, VBX_E_STATE, "no ESDF layer");
-  if (int rc = refresh_host_mirror(c)) return rc;
-  std::vector<uint8_t> upd, has;
-  if (int rc = fetch_flags(c, layer, &upd, &has)) return rc;
+  LayerSlots view;
+  if (int rc = read_layer_slots(c, layer, &view)) return rc;
+  std::vector<int32_t> slots(m);
+  view.find(idx3, m, slots.data());
   const size_t vbytes = (layer == VBX_LAYER_TSDF) ? sizeof(TsdfVoxel) : sizeof(EsdfVoxel);
   const size_t bbytes = vbytes * c->vox_per_block;
   const char* pool = (layer == VBX_LAYER_TSDF) ? reinterpret_cast<const char*>(c->tab.tsdf)
                                                : reinterpret_cast<const char*>(c->tab.esdf);
   for (uint64_t i = 0; i < m; ++i) {
-    auto it = c->host_key2slot.find(pack3(idx3[3 * i], idx3[3 * i + 1], idx3[3 * i + 2]));
-    if (it == c->host_key2slot.end() || !has[it->second]) return fail(c, VBX_E_NOT_FOUND, "block not allocated");
-    VBX_CUDA(c, cudaMemcpyAsync(static_cast<char*>(voxels) + i * bbytes, pool + (size_t)it->second * bbytes,
+    if (slots[i] < 0) return fail(c, VBX_E_NOT_FOUND, "block not allocated");
+    // one copy per block: the mirror's gather kernels are tested against this path
+    VBX_CUDA(c, cudaMemcpyAsync(static_cast<char*>(voxels) + i * bbytes, pool + (size_t)slots[i] * bbytes,
                                 bbytes, cudaMemcpyDeviceToHost, c->stream));
-    if (updated_bits) updated_bits[i] = upd[it->second];
+    if (updated_bits) updated_bits[i] = view.flags[slots[i]] & kReportedBits;
   }
   VBX_CUDA(c, cudaStreamSynchronize(c->stream));
   return VBX_OK;
@@ -832,15 +790,8 @@ int vbx_clear_updated(vbx_ctx* c, int layer, int updated_mask) {
   if (!c) return VBX_E_INVALID;
   VBX_CUDA(c, cudaSetDevice(c->device));
   VBX_DRAIN(c);
-  if (c->n_blocks == 0) return VBX_OK;
-  std::vector<uint8_t> upd(c->n_blocks);
-  uint8_t* dst = (layer == VBX_LAYER_TSDF) ? c->tab.slot_updated : c->tab.slot_esdf_updated;
-  VBX_CUDA(c, cudaMemcpyAsync(upd.data(), dst, c->n_blocks, cudaMemcpyDeviceToHost, c->stream));
-  VBX_CUDA(c, cudaStreamSynchronize(c->stream));
-  for (uint8_t& u : upd) u &= (uint8_t)(~updated_mask | 0x80);  // bit 7 is the engine's own (kSlotNoTsdf / kEsdfPending)
-  VBX_CUDA(c, cudaMemcpyAsync(dst, upd.data(), c->n_blocks, cudaMemcpyHostToDevice, c->stream));
-  VBX_CUDA(c, cudaStreamSynchronize(c->stream));
-  return VBX_OK;
+  return keep_flag_bits(c, (layer == VBX_LAYER_TSDF) ? c->tab.slot_updated : c->tab.slot_esdf_updated,
+                        (uint8_t)(~updated_mask | kEngineBit));
 }
 
 int vbx_upload_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, const void* voxels,

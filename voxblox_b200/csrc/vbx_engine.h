@@ -35,11 +35,14 @@ constexpr size_t kApproxSetWords = (1u << 20) + kApproxSetResets;
 //     Any TSDF touch writes the byte to 7 (Block::updated().set()), which turns the slot into a TSDF block
 //     that starts from zeroed voxels, exactly like a freshly allocated one.
 //   slot_esdf_updated bit 7: member of EsdfIntegrator::updated_blocks_ (esdf_integrator.h:172-175).
-constexpr uint8_t kSlotNoTsdf = 0x80, kEsdfPending = 0x80;
+constexpr uint8_t kEngineBit = 0x80;  // bit 7 of either byte: no caller selects, clears or is told about it
+constexpr uint8_t kSlotNoTsdf = kEngineBit, kEsdfPending = kEngineBit;
 //   bit 3 of both flag bytes (VBX_UPDATED_MIRROR): the block changed since a vbx_mirror_updated /
 //     vbx_serialize_updated call last cleared this bit -- the engine's own dirty mark for the incremental
 //     host mirror, independent of the three Block::updated() bits (which their consumers clear).
 constexpr uint8_t kTouchedBits = 0x0F;  // what a TSDF update writes: Block::updated().set() + the mirror mark
+constexpr uint8_t kReportedBits = 0x07;  // Block::updated() (kMap | kMesh | kEsdf): the bits the C-ABI reports
+constexpr uint8_t kMirrorBits = 0x7F;    // what a mirror call may select on or clear: all but kEngineBit
 
 struct EsdfVoxel {  // core/voxel.h:18-37
   float distance;
@@ -375,6 +378,29 @@ namespace vbx {
 int fail(vbx_ctx* c, int code, const std::string& msg);
 int cuda_fail(vbx_ctx* c, cudaError_t e, const char* what);
 int refresh_host_mirror(vbx_ctx* c);
+
+// One layer's view of the pool slots (read_layer_slots): every host caller that asks which slots hold a
+// block of the layer, with which flag bits, reads it here.  The TSDF and the ESDF layer share pool slots; a
+// slot belongs to the TSDF layer unless its slot_updated carries kSlotNoTsdf, and to the ESDF layer when
+// slot_has_esdf is set (a slot may hold both, either or, after a batch ESDF update wiped an ESDF-only
+// block, neither).  Valid until the next call that changes the pool.
+struct LayerSlots {
+  struct Entry {
+    int x, y, z;
+    uint32_t slot;
+  };
+  const vbx_ctx* c = nullptr;
+  std::vector<uint8_t> flags;   // [n_blocks] the layer's raw flag byte (slot_updated / slot_esdf_updated)
+  std::vector<uint8_t> member;  // [n_blocks] 1: the layer holds a block in this slot
+  // The member slots with (flags & select_bits & mask) != 0, or every member when mask == 0, by (x, y, z)
+  std::vector<Entry> sorted(uint8_t select_bits, int mask) const;
+  // slots_out[i] = the slot of block idx3[i], or -1 when the layer holds no block there
+  void find(const int32_t* idx3, uint64_t m, int32_t* slots_out) const;
+};
+// The host mirror of slot_key brought up to date, then the layer's flag bytes (and slot_has_esdf) in one read
+int read_layer_slots(vbx_ctx* c, int layer, LayerSlots* view);
+// flags[s] &= keep over the slots in use, on the main stream
+int keep_flag_bits(vbx_ctx* c, uint8_t* flags, uint8_t keep);
 int mirror_updated(vbx_ctx* c, int layer, int updated_mask, int clear_mask, int32_t* idx3, void* voxels,
                    uint8_t* updated_bits, uint64_t cap, uint64_t* n, int serialized);
 int esdf_destroy(vbx_ctx* c);

@@ -795,14 +795,7 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
 // EsdfIntegrator::clear(), esdf_integrator.h:135-140: forget the work addNewRobotPosition queued
 int esdf_clear_state(vbx_ctx* c) {
   c->esdf_pending_raise = c->esdf_pending_open = 0;
-  if (c->n_blocks == 0) return VBX_OK;
-  std::vector<uint8_t> eu(c->n_blocks);
-  VBX_CUDA(c, cudaMemcpyAsync(eu.data(), c->tab.slot_esdf_updated, c->n_blocks, cudaMemcpyDeviceToHost, c->stream));
-  VBX_CUDA(c, cudaStreamSynchronize(c->stream));
-  for (uint8_t& u : eu) u &= (uint8_t)~kEsdfPending;
-  VBX_CUDA(c, cudaMemcpyAsync(c->tab.slot_esdf_updated, eu.data(), c->n_blocks, cudaMemcpyHostToDevice, c->stream));
-  VBX_CUDA(c, cudaStreamSynchronize(c->stream));
-  return VBX_OK;
+  return keep_flag_bits(c, c->tab.slot_esdf_updated, (uint8_t)~kEsdfPending);
 }
 
 // EsdfIntegrator::addNewRobotPosition(position), esdf_integrator.cc:25-92
@@ -884,19 +877,17 @@ int esdf_update(vbx_ctx* c, int batch, int clear_updated_flag) {
 // EsdfIntegrator::updateFromTsdfBlocks(tsdf_blocks, incremental), esdf_integrator.cc:124-302: blocks
 // without a TSDF block are skipped (cc:139-141); a block listed twice is processed once.
 int esdf_update_blocks(vbx_ctx* c, const int32_t* idx3, uint64_t m, int incremental) {
-  if (int rc = refresh_host_mirror(c)) return rc;
+  LayerSlots tsdf;
+  if (int rc = read_layer_slots(c, VBX_LAYER_TSDF, &tsdf)) return rc;
+  std::vector<int32_t> found(m);
+  tsdf.find(idx3, m, found.data());
   std::vector<uint32_t> slots;
   slots.reserve(m);
-  std::vector<uint8_t> seen(c->n_blocks, 0), upd(c->n_blocks, 0);
-  if (c->maybe_esdf_only && c->n_blocks) {
-    VBX_CUDA(c, cudaMemcpyAsync(upd.data(), c->tab.slot_updated, c->n_blocks, cudaMemcpyDeviceToHost, c->stream));
-    VBX_CUDA(c, cudaStreamSynchronize(c->stream));
-  }
-  for (uint64_t i = 0; i < m; ++i) {
-    auto it = c->host_key2slot.find(pack3(idx3[3 * i], idx3[3 * i + 1], idx3[3 * i + 2]));
-    if (it == c->host_key2slot.end() || seen[it->second] || (upd[it->second] & kSlotNoTsdf)) continue;
-    seen[it->second] = 1;
-    slots.push_back((uint32_t)it->second);
+  std::vector<uint8_t> seen(c->n_blocks, 0);
+  for (int32_t sl : found) {
+    if (sl < 0 || seen[sl]) continue;
+    seen[sl] = 1;
+    slots.push_back((uint32_t)sl);
   }
   return esdf_run(c, 0, incremental ? 1 : 0, 0, slots.data(), (uint32_t)slots.size());
 }

@@ -313,30 +313,12 @@ int mesh_generate(vbx_ctx* c, const vbx_mesh_config* cfg, int only_updated, int 
   if (n_blocks_out) *n_blocks_out = 0;
   if (n_vertices_out) *n_vertices_out = 0;
   if (c->n_blocks == 0) return VBX_OK;
-  if (int rc = refresh_host_mirror(c)) return rc;
-  // getAllUpdatedBlocks(Update::kMesh) / getAllAllocatedBlocks of the TSDF layer, sorted by index
-  std::vector<uint8_t> upd(c->n_blocks);
-  VBX_CUDA(c, cudaMemcpyAsync(upd.data(), c->tab.slot_updated, c->n_blocks, cudaMemcpyDeviceToHost, s));
-  VBX_CUDA(c, cudaStreamSynchronize(s));
-  struct Item {
-    int x, y, z;
-    uint32_t slot;
-  };
-  std::vector<Item> items;
-  for (uint32_t sl = 0; sl < c->n_blocks; ++sl) {
-    if (upd[sl] & kSlotNoTsdf) continue;
-    if (only_updated && !(upd[sl] & VBX_UPDATED_MESH)) continue;
-    Item it;
-    unpack3(c->host_slot_key[sl], &it.x, &it.y, &it.z);
-    it.slot = sl;
-    items.push_back(it);
-  }
+  // getAllUpdatedBlocks(Update::kMesh) / getAllAllocatedBlocks of the TSDF layer, sorted by index (the mesher
+  // reads the TSDF layer only: a slot that holds an ESDF block alone gets no mesh)
+  LayerSlots view;
+  if (int rc = read_layer_slots(c, VBX_LAYER_TSDF, &view)) return rc;
+  const std::vector<LayerSlots::Entry> items = view.sorted(VBX_UPDATED_MESH, only_updated ? VBX_UPDATED_MESH : 0);
   if (items.empty()) return VBX_OK;
-  std::sort(items.begin(), items.end(), [](const Item& a, const Item& b) {
-    if (a.x != b.x) return a.x < b.x;
-    if (a.y != b.y) return a.y < b.y;
-    return a.z < b.z;
-  });
   const uint32_t nb = (uint32_t)items.size();
   if (nb > c->mesh_cap_blocks) {
     const uint64_t want = std::max<uint64_t>(2ull * nb, 256);
