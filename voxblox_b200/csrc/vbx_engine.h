@@ -58,7 +58,6 @@ enum : uint32_t {
   kErrCoordRange = 4u,      // |voxel coordinate| >= 2^20 * vps
   kErrUpdatesFull = 8u,     // ray-voxel updates exceed max_updates_per_pass
   kFatalErrors = 15u,       // any of the above
-  kErrParentRange = 16u,    // ESDF, full-Euclidean mode: a parent vector component outside [-512, 511]
   kSkipped = 32u,           // not an error: the scan was queued behind a scan that must be redone (vbx_capi.cu)
 };
 
@@ -93,19 +92,13 @@ struct ScanState {
   uint32_t n_blocks;         // pool slots in use after the call
   unsigned long long total_updates;  // K the back half runs on (0 when the call failed / is redone)
   unsigned long long total_found;    // K as counted
-  // ESDF
-  uint32_t esdf_counts[7];
-  uint32_t raise_n2;         // third raise-level counter (see esdf_cnt: the counters rotate mod 3)
-  uint32_t frontier_n[2];
-  uint32_t raise_n[2];
-  uint32_t seed_n;           // ESDF: new free voxels waiting for updateVoxelFromNeighbors
-  uint32_t lowered_n;        // ESDF: voxels lowered by the wavefront
   uint32_t n_ray_list;       // bundle heads (Merged)
   uint32_t n_long;           // voxel runs longer than kShortRun updates (k_apply_prep's long-run list)
   uint32_t long_ticket;      // k_apply: long runs handed out
   uint32_t n_refold;         // bundles folded a second time with IEEE division (diagnostic)
   uint32_t refold_members;   // ... and the points they hold
-  uint32_t frontier_n2;      // third wavefront counter
+  uint32_t tile_ticket;      // k_apply: record tiles of the short runs handed out
+  uint32_t apply_paths[12];  // k_apply: how often each arithmetic path ran, summed over the call (ApplyPath)
   // Merged: bounding box of the valid points' voxels, both ends atomicMax'ed (so that an all-zero
   // block means "no valid point"): kb_max = v + 2^30, kb_min = 0xffffffff - (v + 2^30); the bundle
   // keys are packed relative to it (vbx_tsdf.cu, KeyLayout)
@@ -116,14 +109,30 @@ struct ScanState {
   uint32_t merge_ticket;     // Merged: work hand-out counter of k_merge
   uint32_t n_touch_ids;      // touched-block ids handed out: one per block the call touches (vbx_hash.cuh)
   uint32_t rec_key_bits;     // bits an update-record key uses: voxel-in-block bits + bits of the touched ids
-  uint32_t esdf_ticket[6];   // ESDF queue kernels: work hand-out counters, rotating like the queue counters ([0..2] raise, [3..5] lower)
-  uint32_t tile_ticket;      // k_apply: record tiles of the short runs handed out
-  uint32_t apply_paths[12];  // k_apply: how often each arithmetic path ran, summed over the call (ApplyPath)
   uint32_t ids_resolved;     // local block ids k_assign has resolved so far in this call (all passes)
-  uint32_t reserved;
 };
-static_assert(sizeof(ScanState) == 256, "the status block the host reads back is 256 bytes");
+static_assert(sizeof(ScanState) == 168, "the status block the host reads back is 168 bytes");
+static_assert(offsetof(ScanState, total_updates) % 8 == 0 && offsetof(ScanState, total_found) % 8 == 0,
+              "64-bit counters stay 8-byte aligned");
 static_assert(sizeof(ScanState::apply_paths) / 4 == kApplyPaths, "one word per apply path");
+
+// Error bits raised on the device (EsdfState::error)
+enum : uint32_t {
+  kEsdfErrQueueFull = 1u,    // a wavefront / raise / seed queue append past its capacity
+  kEsdfErrParentRange = 2u,  // full-Euclidean mode: a parent vector component outside [-512, 511]
+};
+
+// The ESDF's per-call status block (vbx_esdf.cu), device-resident; the host reads it back through pinned memory.
+struct EsdfState {
+  uint32_t error;
+  uint32_t counts[7];      // [0] blocks listed, [1..6] the VLOG counters (vbx_esdf_get_counters)
+  // The queue kernels rotate through three counters per queue: sweep k reads [k % 3], appends to
+  // [(k + 1) % 3] and zeroes [(k + 2) % 3], so a sweep needs one grid-wide barrier.
+  uint32_t frontier_n[3];  // the open queue (wavefront)
+  uint32_t raise_n[3];     // the raise queue
+  uint32_t seed_n;         // new free voxels waiting for updateVoxelFromNeighbors
+  uint32_t lowered_n;      // voxels lowered by the wavefront
+};
 
 // The GPU-resident block hash + voxel pools (the device mirror of Layer<T>::block_map_,
 // core/layer.h:30-32,292).
@@ -335,7 +344,9 @@ struct vbx_ctx {
   // full-Euclidean mode only (allocated by its first update): every voxel's distance and parent as one 64-bit
   // word, so that the wavefront lowers both in a single atomicMin (vbx_esdf.cu, fe_pack)
   unsigned long long* esdf_fe = nullptr;
-  int esdf_grid_raise = 0, esdf_grid_lower = 0, esdf_sms = 0, esdf_ctas_wide = 1, esdf_ctas_small = 1;
+  vbx::EsdfState* esdf_d_state = nullptr;
+  vbx::EsdfState* esdf_h_state = nullptr;  // page-locked
+  int esdf_sms = 0, esdf_ctas_wide = 1;
   uint32_t esdf_pending_raise = 0, esdf_pending_open = 0;  // raise_ / open_ entries queued by addNewRobotPosition
   bool maybe_esdf_only = false;                            // some slot may carry kSlotNoTsdf
   // mesher (vbx_mesh.cu): the result of the last vbx_mesh_generate stays on the device until the next one

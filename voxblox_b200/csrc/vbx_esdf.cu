@@ -116,23 +116,13 @@ __device__ __forceinline__ void mark_mirror(const Tables& tab, int L, uint32_t r
   if (!(*f & 8)) *f |= 8;  // (every concurrent writer stores the same bit)
 }
 
-__device__ __forceinline__ void push(uint32_t* list, uint32_t* count, uint32_t cap, uint32_t ref, ScanState* st) {
+__device__ __forceinline__ void push(uint32_t* list, uint32_t* count, uint32_t cap, uint32_t ref, EsdfState* st) {
   const uint32_t j = atomicAdd(count, 1u);
   if (j < cap) {
     list[j] = ref;
   } else {
-    atomicOr(&st->error, kErrUpdatesFull);
+    atomicOr(&st->error, kEsdfErrQueueFull);
   }
-}
-
-// The level-synchronous kernels below keep THREE counters per queue and rotate through them: sweep k
-// reads counter k % 3, appends to counter (k + 1) % 3 and zeroes counter (k + 2) % 3 (last read one
-// sweep ago, next written one sweep ahead), so a sweep needs a single grid-wide barrier.
-__device__ __forceinline__ uint32_t* frontier_cnt(ScanState* st, uint32_t k) {
-  return k % 3u == 2u ? &st->frontier_n2 : &st->frontier_n[k % 3u];
-}
-__device__ __forceinline__ uint32_t* raise_cnt(ScanState* st, uint32_t k) {
-  return k % 3u == 2u ? &st->raise_n2 : &st->raise_n[k % 3u];
 }
 
 // Step (1), esdf_integrator.cc:136-287, for ONE voxel: the stored ESDF voxel `ev` against its TSDF voxel `tv`.
@@ -217,7 +207,7 @@ __device__ __forceinline__ bool esdf_classify(const EsdfParams& E, const TsdfVox
 }
 
 // one queue append per warp instead of one per voxel
-__device__ __forceinline__ void push_warp(bool want, uint32_t* list, uint32_t* count, uint32_t cap, uint32_t ref, ScanState* st) {
+__device__ __forceinline__ void push_warp(bool want, uint32_t* list, uint32_t* count, uint32_t cap, uint32_t ref, EsdfState* st) {
   const unsigned m = __ballot_sync(0xffffffffu, want);
   if (!m) return;
   const int lane = threadIdx.x & 31;
@@ -229,7 +219,7 @@ __device__ __forceinline__ void push_warp(bool want, uint32_t* list, uint32_t* c
     if (j < cap) {
       list[j] = ref;
     } else {
-      atomicOr(&st->error, kErrUpdatesFull);
+      atomicOr(&st->error, kEsdfErrQueueFull);
     }
   }
 }
@@ -278,15 +268,15 @@ __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.a
 // 20 B in/out per voxel.  One thread block per voxel block: the TSDF slab (48 KiB at 16^3) and the ESDF slab
 // (80 KiB) are staged into shared memory by two TMA bulk copies, classified from there (every thread a few
 // voxels), and the ESDF slab goes back with one bulk store.  Queue appends are warp-aggregated, the VLOG
-// counters block-aggregated.  esdf_counts: [1] lower [2] raise [3] new.
+// counters block-aggregated.  counts: [1] lower [2] raise [3] new.
 __global__ void __launch_bounds__(1024)
 k_esdf_propagate(EsdfParams E, Tables tab, const uint32_t* __restrict__ block_list, uint32_t n_blocks,
-                 uint32_t* open_list, uint32_t* raise_list, uint32_t* seed_list, ScanState* st) {
+                 uint32_t* open_list, uint32_t* raise_list, uint32_t* seed_list, EsdfState* st) {
   extern __shared__ __align__(128) unsigned char slab[];
   __shared__ __align__(8) uint64_t bar;
   __shared__ uint32_t s_cnt[4];
   const uint32_t vpb = 1u << (3 * E.L);
-  if (blockIdx.x >= min(n_blocks, st->esdf_counts[0])) return;  // (n_blocks is the launch's upper bound)
+  if (blockIdx.x >= min(n_blocks, st->counts[0])) return;  // (n_blocks is the launch's upper bound)
   const uint32_t slot = block_list[blockIdx.x];
   TsdfVoxel* s_tsdf = reinterpret_cast<TsdfVoxel*>(slab);
   EsdfWords* s_esdf = reinterpret_cast<EsdfWords*>(slab + (size_t)vpb * sizeof(TsdfVoxel));
@@ -344,7 +334,7 @@ k_esdf_propagate(EsdfParams E, Tables tab, const uint32_t* __restrict__ block_li
   } else {
     for (uint32_t lin = threadIdx.x; lin < vpb; lin += blockDim.x) g_esdf[lin] = s_esdf[lin];
   }
-  if (threadIdx.x >= 1 && threadIdx.x < 4 && s_cnt[threadIdx.x]) atomicAdd(&st->esdf_counts[threadIdx.x], s_cnt[threadIdx.x]);
+  if (threadIdx.x >= 1 && threadIdx.x < 4 && s_cnt[threadIdx.x]) atomicAdd(&st->counts[threadIdx.x], s_cnt[threadIdx.x]);
 }
 
 // updateVoxelFromNeighbors (cc:498-530) for the new free-space voxels of an incremental update:
@@ -353,7 +343,7 @@ k_esdf_propagate(EsdfParams E, Tables tab, const uint32_t* __restrict__ block_li
 // their post-classification state (the reference sees neighbours seeded earlier in its own
 // loop order as well; see DESIGN.md).
 __global__ void k_esdf_seed(EsdfParams E, Tables tab, const uint32_t* __restrict__ seed_list, uint32_t* open_list,
-                            float* seed_val, ScanState* st) {
+                            float* seed_val, EsdfState* st) {
   const uint32_t n = min(st->seed_n, E.cap);
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const uint32_t ref = seed_list[i];
@@ -382,7 +372,7 @@ __global__ void k_esdf_seed(EsdfParams E, Tables tab, const uint32_t* __restrict
 }
 
 __global__ void k_esdf_seed_commit(EsdfParams E, Tables tab, const uint32_t* __restrict__ seed_list,
-                                   const float* __restrict__ seed_val, const ScanState* st) {
+                                   const float* __restrict__ seed_val, const EsdfState* st) {
   const uint32_t n = min(st->seed_n, E.cap);
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     (reinterpret_cast<EsdfWords*>(tab.esdf) + seed_list[i])->distance = seed_val[i];
@@ -393,7 +383,7 @@ __global__ void k_esdf_seed_commit(EsdfParams E, Tables tab, const uint32_t* __r
 // lane per neighbour.  A neighbour whose parent points back at the raised voxel is reset and
 // raised in turn; any other observed, non-fixed neighbour joins the open set.
 __global__ void k_esdf_raise(EsdfParams E, Tables tab, uint32_t* raise_a, uint32_t* raise_b, uint32_t* open_list,
-                             ScanState* st) {
+                             EsdfState* st) {
   cg::grid_group grid = cg::this_grid();
   const int lane = threadIdx.x & 31;
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -401,13 +391,13 @@ __global__ void k_esdf_raise(EsdfParams E, Tables tab, uint32_t* raise_a, uint32
   for (uint32_t level = 0;; ++level) {
     uint32_t* in = (level & 1u) ? raise_b : raise_a;
     uint32_t* out = (level & 1u) ? raise_a : raise_b;
-    const uint32_t n = min(__ldcg(raise_cnt(st, level)), E.cap);
+    const uint32_t n = min(__ldcg(&st->raise_n[level % 3u]), E.cap);
     if (n == 0) break;
-    uint32_t* out_n = raise_cnt(st, level + 1);
-    if (blockIdx.x == 0 && threadIdx.x == 0) *raise_cnt(st, level + 2) = 0;
+    uint32_t* out_n = &st->raise_n[(level + 1) % 3u];
+    if (blockIdx.x == 0 && threadIdx.x == 0) st->raise_n[(level + 2) % 3u] = 0;
     for (uint32_t q = warp; q < n; q += n_warps) {
       const uint32_t ref = __ldcg(&in[q]);
-      if (lane == 0) atomicAdd(&st->esdf_counts[4], 1u);
+      if (lane == 0) atomicAdd(&st->counts[4], 1u);
       if (lane < 26) {
         const uint32_t nref = neighbor_ref(tab, E.L, ref, lane);
         if (nref != 0xffffffffu) {
@@ -460,10 +450,10 @@ __device__ __forceinline__ void fe_parent(long long w, int* x, int* y, int* z) {
 }
 
 // full-Euclidean mode, before the wavefront: every voxel's (distance, parent) into its 64-bit word
-__global__ void k_esdf_fe_pack(Tables tab, uint64_t nvox, long long* fe, ScanState* st) {
+__global__ void k_esdf_fe_pack(Tables tab, uint64_t nvox, long long* fe, EsdfState* st) {
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nvox; i += (uint64_t)gridDim.x * blockDim.x) {
     const EsdfWords& e = reinterpret_cast<const EsdfWords*>(tab.esdf)[i];
-    if (!fe_parent_ok(e.px, e.py, e.pz)) atomicOr(&st->error, kErrParentRange);
+    if (!fe_parent_ok(e.px, e.py, e.pz)) atomicOr(&st->error, kEsdfErrParentRange);
     fe[i] = fe_pack(e.distance, e.px, e.py, e.pz);
   }
 }
@@ -476,7 +466,7 @@ __global__ void k_esdf_fe_pack(Tables tab, uint64_t nvox, long long* fe, ScanSta
 // fe: nullptr in quasi-Euclidean mode; in full-Euclidean mode the packed (distance, parent) words, which
 // stand in for the voxels' distance and parent fields until k_esdf_parents writes them back.
 __global__ void k_esdf_lower(EsdfParams E, Tables tab, uint32_t* front_a, uint32_t* front_b, uint32_t* touched_list,
-                             long long* fe, ScanState* st) {
+                             long long* fe, EsdfState* st) {
   cg::grid_group grid = cg::this_grid();
   const int lane = threadIdx.x & 31;
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -484,12 +474,12 @@ __global__ void k_esdf_lower(EsdfParams E, Tables tab, uint32_t* front_a, uint32
   for (uint32_t sweep = 0;; ++sweep) {
     uint32_t* in = (sweep & 1u) ? front_b : front_a;
     uint32_t* out = (sweep & 1u) ? front_a : front_b;
-    const uint32_t n = min(__ldcg(frontier_cnt(st, sweep)), E.cap);
+    const uint32_t n = min(__ldcg(&st->frontier_n[sweep % 3u]), E.cap);
     if (n == 0) break;
-    uint32_t* out_n = frontier_cnt(st, sweep + 1);
+    uint32_t* out_n = &st->frontier_n[(sweep + 1) % 3u];
     if (blockIdx.x == 0 && threadIdx.x == 0) {
-      *frontier_cnt(st, sweep + 2) = 0;
-      atomicAdd(&st->esdf_counts[6], 1u);
+      st->frontier_n[(sweep + 2) % 3u] = 0;
+      atomicAdd(&st->counts[6], 1u);
     }
     for (uint32_t q = warp; q < n; q += n_warps) {
       const uint32_t ref = __ldcg(&in[q]);
@@ -524,7 +514,7 @@ __global__ void k_esdf_lower(EsdfParams E, Tables tab, uint32_t* front_a, uint32
                                        norm3(f3((float)vpx, (float)vpy, (float)vpz))));
         if (dist < 0.0f) continue;
         if (!fe_parent_ok(npx, npy, npz)) {
-          atomicOr(&st->error, kErrParentRange);
+          atomicOr(&st->error, kEsdfErrParentRange);
           continue;
         }
       }
@@ -554,7 +544,7 @@ __global__ void k_esdf_lower(EsdfParams E, Tables tab, uint32_t* front_a, uint32
         }
       }
       if (changed) {
-        atomicAdd(&st->esdf_counts[5], 1u);
+        atomicAdd(&st->counts[5], 1u);
         mark_mirror(tab, E.L, nref);
         // neighbor_voxel->parent = new_parent (cc:436,450,470,481).  Full-Euclidean mode: it went into the
         // packed word with the distance.  Quasi-Euclidean mode: written unguarded, when two sources lower the
@@ -581,7 +571,7 @@ __global__ void k_esdf_lower(EsdfParams E, Tables tab, uint32_t* front_a, uint32
 // with equal candidates that is its visiting order.)  Full-Euclidean mode: the distance and parent
 // the wavefront left in the voxel's packed word.
 __global__ void k_esdf_parents(EsdfParams E, Tables tab, const uint32_t* __restrict__ touched_list,
-                               const long long* __restrict__ fe, ScanState* st) {
+                               const long long* __restrict__ fe, EsdfState* st) {
   const uint32_t n = min(st->lowered_n, E.cap);
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const uint32_t ref = touched_list[i];
@@ -619,7 +609,7 @@ __global__ void k_esdf_parents(EsdfParams E, Tables tab, const uint32_t* __restr
 // (updated_blocks_, cc:104-110) -- incremental -- or every TSDF block (batch).  Slots that hold an
 // ESDF block only (kSlotNoTsdf) are skipped like the reference skips indices without a TSDF
 // block (cc:137-141).
-__global__ void k_esdf_block_list(Tables tab, uint32_t n_slots, int batch, uint32_t* block_list, ScanState* st) {
+__global__ void k_esdf_block_list(Tables tab, uint32_t n_slots, int batch, uint32_t* block_list, EsdfState* st) {
   const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= n_slots) return;
   const uint8_t u = tab.slot_updated[s];
@@ -627,7 +617,7 @@ __global__ void k_esdf_block_list(Tables tab, uint32_t n_slots, int batch, uint3
   if (eu & kEsdfPending) tab.slot_esdf_updated[s] = eu & (uint8_t)~kEsdfPending;  // updated_blocks_.clear(), cc:99,109
   if (u & kSlotNoTsdf) return;
   if (batch || (u & VBX_UPDATED_ESDF) || (eu & kEsdfPending)) {
-    block_list[atomicAdd(&st->esdf_counts[0], 1u)] = s;
+    block_list[atomicAdd(&st->counts[0], 1u)] = s;
     tab.slot_has_esdf[s] = 1;  // allocateBlockPtrByIndex in the ESDF layer, cc:143-146
     tab.slot_esdf_updated[s] = (tab.slot_esdf_updated[s] & kEsdfPending) | 9;  // esdf_block->set_updated(true): bitset(1) = kMap only, cc:147 (+ the mirror mark)
   }
@@ -686,7 +676,7 @@ __global__ void k_esdf_sphere_blocks(SphereParams S, ScanBlocks sb, const float*
 }
 
 __global__ void k_esdf_sphere_apply(SphereParams S, Tables tab, const float* __restrict__ xs, uint32_t* raise_list,
-                                    uint32_t* open_list, ScanState* st) {
+                                    uint32_t* open_list, EsdfState* st) {
   int gx, gy, gz;
   if (!sphere_voxel(S, xs, (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, &gx, &gy, &gz)) return;
   const uint32_t hp = find_block(tab, pack3(gx >> S.L, gy >> S.L, gz >> S.L));
@@ -720,18 +710,18 @@ __global__ void k_esdf_sphere_apply(SphereParams S, Tables tab, const float* __r
     if ((tab.slot_esdf_updated[slot] & (kEsdfPending | 8)) != (kEsdfPending | 8)) {
       tab.slot_esdf_updated[slot] |= (uint8_t)(kEsdfPending | 8);  // updated_blocks_.insert (+ the mirror mark)
     }
-    atomicAdd(&st->esdf_counts[S.outer ? 2 : 1], 1u);
+    atomicAdd(&st->counts[S.outer ? 2 : 1], 1u);
   }
 }
 
-__global__ void k_esdf_set_pending(ScanState* st, uint32_t n_raise, uint32_t n_open) {
+__global__ void k_esdf_set_pending(EsdfState* st, uint32_t n_raise, uint32_t n_open) {
   st->raise_n[0] = n_raise;
   st->frontier_n[0] = n_open;
 }
 
-__global__ void k_esdf_clear_tsdf_flag(Tables tab, const uint32_t* __restrict__ block_list, const ScanState* st) {
+__global__ void k_esdf_clear_tsdf_flag(Tables tab, const uint32_t* __restrict__ block_list, const EsdfState* st) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= st->esdf_counts[0]) return;
+  if (i >= st->counts[0]) return;
   tab.slot_updated[block_list[i]] &= (uint8_t)~VBX_UPDATED_ESDF;  // cc:113-121
 }
 
@@ -739,11 +729,13 @@ static inline unsigned int grid_for(uint64_t n, int block) { return (unsigned in
 
 int esdf_destroy(vbx_ctx* c) {
   void* ptrs[] = {c->tab.esdf, c->frontier[0], c->frontier[1], c->raise_q[0], c->raise_q[1], c->esdf_block_list,
-                  c->esdf_seed_list, c->esdf_seed_val, c->esdf_touched, c->esdf_fe};
+                  c->esdf_seed_list, c->esdf_seed_val, c->esdf_touched, c->esdf_fe, c->esdf_d_state};
   for (void* p : ptrs) {
     if (p) cudaFree(p);
   }
+  if (c->esdf_h_state) cudaFreeHost(c->esdf_h_state);
   c->esdf_fe = nullptr;
+  c->esdf_d_state = c->esdf_h_state = nullptr;
   c->tab.esdf = nullptr;
   c->frontier[0] = c->frontier[1] = c->raise_q[0] = c->raise_q[1] = c->esdf_block_list = nullptr;
   c->esdf_seed_list = c->esdf_touched = nullptr;
@@ -770,6 +762,8 @@ int esdf_create(vbx_ctx* c, const vbx_esdf_config* cfg) {
   VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_seed_list), c->frontier_cap * sizeof(uint32_t)));
   VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_seed_val), c->frontier_cap * sizeof(float)));
   VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_touched), c->frontier_cap * sizeof(uint32_t)));
+  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_d_state), sizeof(EsdfState)));
+  VBX_CUDA(c, cudaMallocHost(reinterpret_cast<void**>(&c->esdf_h_state), sizeof(EsdfState)));
   int dev = c->device, sms = 0, per_sm_r = 0, per_sm_l = 0;
   VBX_CUDA(c, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   VBX_CUDA(c, cudaFuncSetAttribute(k_esdf_propagate, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -782,8 +776,6 @@ int esdf_create(vbx_ctx* c, const vbx_esdf_config* cfg) {
   // updates over many blocks (batch mode, LiDAR) get the wider grid, see esdf_run
   c->esdf_sms = sms;
   c->esdf_ctas_wide = std::max(1, std::min(std::min(per_sm_r, per_sm_l), 4));
-  c->esdf_grid_raise = sms;
-  c->esdf_grid_lower = sms;
   VBX_CUDA(c, cudaStreamSynchronize(c->stream));
   c->has_esdf = true;
   return VBX_OK;
@@ -825,11 +817,15 @@ int esdf_add_robot_position(vbx_ctx* c, const float p[3]) {
   }
   // the per-axis lists ride in the seed-value scratch (floats; frontier_cap >> 1300 entries)
   float* d_xs[2] = {c->esdf_seed_val, c->esdf_seed_val + xs[0].size()};
-  const vbx_ctx::ScratchSet& set0 = c->set[0];  // hand-off set 0's block table and status block
+  // block creation: hand-off set 0's block table and status block, as for an upload
+  const vbx_ctx::ScratchSet& set0 = c->set[0];
   ScanState* d_state = set0.d_state;
+  // the sphere's voxels, queue appends and counters
+  EsdfState* d_es = c->esdf_d_state;
   VBX_CUDA(c, cudaEventRecord(c->ev0, s));
   VBX_CUDA(c, cudaMemsetAsync(d_state, 0, sizeof(ScanState), s));
-  k_esdf_set_pending<<<1, 1, 0, s>>>(d_state, c->esdf_pending_raise, c->esdf_pending_open);
+  VBX_CUDA(c, cudaMemsetAsync(d_es, 0, sizeof(EsdfState), s));
+  k_esdf_set_pending<<<1, 1, 0, s>>>(d_es, c->esdf_pending_raise, c->esdf_pending_open);
   ++tally.launches;
   for (int k = 0; k < 2; ++k) {
     if (S[k].n == 0) continue;
@@ -844,27 +840,29 @@ int esdf_add_robot_position(vbx_ctx* c, const float p[3]) {
   for (int k = 0; k < 2; ++k) {
     if (S[k].n == 0) continue;
     const uint64_t n3 = (uint64_t)S[k].n * S[k].n * S[k].n;
-    k_esdf_sphere_apply<<<grid_for(n3, 256), 256, 0, s>>>(S[k], c->tab, d_xs[k], c->raise_q[0], c->frontier[0], d_state);
+    k_esdf_sphere_apply<<<grid_for(n3, 256), 256, 0, s>>>(S[k], c->tab, d_xs[k], c->raise_q[0], c->frontier[0], d_es);
     ++tally.launches;
   }
   VBX_CUDA(c, cudaEventRecord(c->ev1, s));
-  VBX_CUDA(c, cudaMemcpyAsync(c->set[0].h_state, d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(set0.h_state, d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(c->esdf_h_state, d_es, sizeof(EsdfState), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));  // (also keeps xs[] alive until the copies are done)
   VBX_CUDA(c, cudaGetLastError());
   VBX_CUDA(c, cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   const ScanState& h = *set0.h_state;
+  const EsdfState& he = *c->esdf_h_state;
   c->n_blocks = h.n_blocks;
   if (h.n_new) c->maybe_esdf_only = true;
   if (h.error & (kErrPoolFull | kErrHashFull)) return check_state_errors(c, h);
   if (h.error & kErrCoordRange) return fail(c, VBX_E_INVALID, "robot position sphere outside the +-2^20 block range");
-  if (h.error & kErrUpdatesFull) return fail(c, VBX_E_CAPACITY, "ESDF wavefront queue capacity exceeded");
-  c->esdf_pending_raise = h.raise_n[0];
-  c->esdf_pending_open = h.frontier_n[0];
+  if (he.error & kEsdfErrQueueFull) return fail(c, VBX_E_CAPACITY, "ESDF wavefront queue capacity exceeded");
+  c->esdf_pending_raise = he.raise_n[0];
+  c->esdf_pending_open = he.frontier_n[0];
   c->esdf_counters[0] = h.n_new;          // ESDF blocks created
-  c->esdf_counters[1] = h.esdf_counts[1]; // voxels set free
-  c->esdf_counters[2] = h.esdf_counts[2]; // voxels set occupied
-  c->esdf_counters[4] = h.raise_n[0];     // queued: raise_
-  c->esdf_counters[5] = h.frontier_n[0];  // queued: open_
+  c->esdf_counters[1] = he.counts[1];     // voxels set free
+  c->esdf_counters[2] = he.counts[2];     // voxels set occupied
+  c->esdf_counters[4] = he.raise_n[0];    // queued: raise_
+  c->esdf_counters[5] = he.frontier_n[0]; // queued: open_
   c->esdf_counters[7] = tally.launches;
   c->launches += tally.launches;
   return refresh_host_mirror(c);
@@ -922,11 +920,11 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
     VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_fe),
                            (size_t)c->tab.max_blocks * c->vox_per_block * sizeof(unsigned long long)));
   }
-  ScanState* d_state = c->set[0].d_state;  // hand-off set 0's status block
-  const ScanState& h = *c->set[0].h_state;
+  EsdfState* d_state = c->esdf_d_state;
+  const EsdfState& h = *c->esdf_h_state;
   VBX_CUDA(c, cudaEventRecord(c->ev0, s));
   tally.begin();
-  VBX_CUDA(c, cudaMemsetAsync(d_state, 0, sizeof(ScanState), s));
+  VBX_CUDA(c, cudaMemsetAsync(d_state, 0, sizeof(EsdfState), s));
   if (c->n_blocks == 0) {
     VBX_CUDA(c, cudaStreamSynchronize(s));
     return VBX_OK;
@@ -956,13 +954,13 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
     nb = n_listed;
     if (nb > 0) {
       VBX_CUDA(c, cudaMemcpyAsync(c->esdf_block_list, listed_slots, (size_t)nb * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-      VBX_CUDA(c, cudaMemcpyAsync(&d_state->esdf_counts[0], &nb, sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+      VBX_CUDA(c, cudaMemcpyAsync(&d_state->counts[0], &nb, sizeof(uint32_t), cudaMemcpyHostToDevice, s));
       k_esdf_mark_listed<<<grid_for(nb, 256), 256, 0, s>>>(c->tab, c->esdf_block_list, nb);
       ++tally.launches;
       VBX_CUDA(c, cudaStreamSynchronize(s));  // the two host sources above are stack / vector memory
     }
   } else {
-    // the list and its length (esdf_counts[0]) stay on the device: no host round trip in the middle of
+    // the list and its length (counts[0]) stay on the device: no host round trip in the middle of
     // the call; the launches below are sized for the upper bound (every slot) and the kernels stop at
     // the real count
     k_esdf_block_list<<<grid_for(c->n_blocks, 256), 256, 0, s>>>(c->tab, c->n_blocks, batch, c->esdf_block_list, d_state);
@@ -985,14 +983,13 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
       ++tally.launches;
     }
     tally.mark(kStageEsdfPropagate);
-    {
-      int per_sm = (nb <= 256 && !pending) ? c->esdf_ctas_small : c->esdf_ctas_wide;
-      if (const char* e = std::getenv("VBX_ESDF_CTAS")) per_sm = std::max(1, std::min(std::atoi(e), c->esdf_ctas_wide));  // (tuning aid)
-      c->esdf_grid_raise = c->esdf_grid_lower = c->esdf_sms * per_sm;
-    }
+    // the persistent grid: one CTA per SM for small incremental updates, the wider grid otherwise (esdf_create)
+    int per_sm = (nb <= 256 && !pending) ? 1 : c->esdf_ctas_wide;
+    if (const char* e = std::getenv("VBX_ESDF_CTAS")) per_sm = std::max(1, std::min(std::atoi(e), c->esdf_ctas_wide));  // (tuning aid)
+    const unsigned int grid = (unsigned int)(c->esdf_sms * per_sm);
     {
       void* args[] = {&E, &c->tab, &c->raise_q[0], &c->raise_q[1], &c->frontier[0], &d_state};
-      VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_esdf_raise, dim3(c->esdf_grid_raise), dim3(256), args, 0, s));
+      VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_esdf_raise, dim3(grid), dim3(256), args, 0, s));
       ++tally.launches;
     }
     tally.mark(kStageEsdfRaise);
@@ -1004,7 +1001,7 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
     }
     {
       void* args[] = {&E, &c->tab, &c->frontier[0], &c->frontier[1], &c->esdf_touched, &fe, &d_state};
-      VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_esdf_lower, dim3(c->esdf_grid_lower), dim3(256), args, 0, s));
+      VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_esdf_lower, dim3(grid), dim3(256), args, 0, s));
       ++tally.launches;
     }
     k_esdf_parents<<<c->grid_sms * 8, 256, 0, s>>>(E, c->tab, c->esdf_touched, fe, d_state);
@@ -1016,16 +1013,16 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
     }
   }
   VBX_CUDA(c, cudaEventRecord(c->ev1, s));
-  VBX_CUDA(c, cudaMemcpyAsync(c->set[0].h_state, d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(c->esdf_h_state, d_state, sizeof(EsdfState), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));
   VBX_CUDA(c, cudaGetLastError());
   VBX_CUDA(c, cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   tally.collect();
-  if (h.error & kErrUpdatesFull) return fail(c, VBX_E_CAPACITY, "ESDF wavefront queue capacity exceeded");
-  if (h.error & kErrParentRange) {
+  if (h.error & kEsdfErrQueueFull) return fail(c, VBX_E_CAPACITY, "ESDF wavefront queue capacity exceeded");
+  if (h.error & kEsdfErrParentRange) {
     return fail(c, VBX_E_CAPACITY, "full-Euclidean ESDF: a parent vector component left [-512, 511] voxels");
   }
-  for (int i = 0; i < 7; ++i) c->esdf_counters[i] = h.esdf_counts[i];
+  for (int i = 0; i < 7; ++i) c->esdf_counters[i] = h.counts[i];
   c->esdf_counters[7] = tally.launches;
   c->launches += tally.launches;
   return VBX_OK;
