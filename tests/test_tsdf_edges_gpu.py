@@ -10,6 +10,9 @@ digests (tests/golden/reference_pins.py), on what the other parity tests never r
    non-constant weights and min_ray_length_m = 0: zero weights, weights below kEpsilon that the Merged fold
    skips, weights near 1e11, big bundles whose weights are all 0 or all near 1e11, a big bundle that the
    Merged fold must fold again with IEEE division, and points within 0.1 m of the sensor;
+ * the bundles whose mean the Merged fold folds again with IEEE division, in each shape that walk meets: fewer
+   than 32 members, the first live member past the first chunk, live and weight-0 members alternating, and a
+   clearing bundle;
  * a truncation distance at or below the voxel size (the weight drop-off's denominator is 0 or negative);
  * max_weight of 1e-7 (a voxel can never rest), 1 and 1e30."""
 import numpy as np
@@ -58,6 +61,29 @@ def _lidar_extreme_z():
     return [(pts, cols, s[2], s[3])]
 
 
+def _refold_cluster(shape):
+    """One scan of one dense cluster with camera-frame x = 0 (so the Merged fold folds its mean again with IEEE
+    division), inside one voxel under C1's pose, shaped for what that refold walks: under 1024 points, so that list
+    order is array order, and weights of 0 at camera-frame z = 0 next to live ones at z ~ 5 mm."""
+    rng = np.random.default_rng(17)
+    F = np.float32
+    jitter = lambda n: rng.uniform(0.0, 1e-4, n).astype(F)
+    live_z = lambda n: F(0.005) + jitter(n)
+    if shape == "short":          # fewer than 32 members: one partial chunk
+        z = F(1.55) + jitter(20)
+    elif shape == "late_live":    # the first live member is past the first chunk
+        z = np.r_[np.zeros(45, F), live_z(60)]
+    elif shape == "alternating":  # live and weight-0 members alternate: partial live masks in every chunk
+        z = np.where(np.arange(100) % 2 == 0, F(0), live_z(100)).astype(F)
+    else:                         # "clearing": beyond max_ray_length_m, so only the first member is taken
+        z = F(6.05) + jitter(50)
+    n = len(z)
+    pts = np.c_[np.zeros(n, F), F(0.55) + jitter(n), z].astype(F)
+    cols = rng.integers(0, 256, (n, 4)).astype(np.uint8)
+    _, _, q, t = scenes.c1_planar_wall()
+    return [(pts, cols, q, t)]
+
+
 def _mutate_prior(words, T, max_weight, seed):
     """Voxels of a serialised block (3 words each) set to the edge states, one in eight of each kind."""
     w = words.reshape(-1, 3).copy()
@@ -90,6 +116,9 @@ CASES["extreme_z/minray0"] = dict(voxel=0.1, cfg=dict(default_truncation_distanc
                                   scans=_lidar_extreme_z, prior=False, paths=[], refold=True)
 CASES["extreme_z/minray0.1"] = dict(voxel=0.1, cfg=dict(default_truncation_distance=0.4, max_ray_length_m=10.0),
                                     scans=_lidar_extreme_z, prior=False, paths=[], refold=True)
+for _shape in ("short", "late_live", "alternating", "clearing"):
+    CASES[f"refold/{_shape}"] = dict(voxel=0.1, cfg=dict(default_truncation_distance=0.4),
+                                     scans=lambda s=_shape: _refold_cluster(s), prior=False, paths=[], refold=True)
 for _f in (1.0, 0.5):
     CASES[f"trunc/c1_wall_x{_f:g}"] = dict(voxel=0.2, cfg=dict(default_truncation_distance=0.2 * _f),
                                            scans=lambda: [scenes.c1_planar_wall()], prior=False, paths=[])
