@@ -231,6 +231,23 @@ VBX_API int vbx_proto_decode_block(const uint8_t* msg, uint64_t len, int32_t* vo
  * (core/layer.h:103-111,152-161); creates the block if needed. */
 VBX_API int vbx_upload_blocks(vbx_ctx* ctx, int layer, const int32_t* idx3, uint64_t m,
                       const void* voxels, const uint8_t* updated_bits);
+/* Device-to-device block transfer, for keeping read-only replicas of a sharded map's other ranks' blocks
+ * (DESIGN.md "multi-GPU").  Both calls take 4-byte aligned DEVICE memory of this context's GPU (cudaMalloc /
+ * torch tensors); host and null pointers give VBX_E_INVALID.
+ * vbx_gather_updated_device: the gather of vbx_mirror_updated into device memory -- every block with
+ * (updated & updated_mask) != 0 (0 = every block), and with owned_only != 0 only the blocks this rank owns
+ * (vbx_block_owner), ascending (x,y,z): d_idx3 receives 3 int32 per block, d_voxels the raw voxel payloads
+ * (the structs above), and clear_mask bits are reset on the device.  Only the block count reaches the host.
+ * *n = number of matching blocks; if *n > cap nothing is copied or cleared (grow and retry). */
+VBX_API int vbx_gather_updated_device(vbx_ctx* ctx, int layer, int updated_mask, int clear_mask, int owned_only,
+                                      int32_t* d_idx3, void* d_voxels, uint64_t cap, uint64_t* n);
+/* vbx_upload_blocks with d_idx3 / d_voxels in device memory: creates the blocks as needed and writes the
+ * payloads straight from d_voxels; every written block's updated() bits become `updated_bits` (the reported
+ * bits only: VBX_UPDATED_MIRROR stays clear).  The indices (12 B per block) are read back to check them before
+ * anything is written.  On a sharded engine (world_size > 1) a block this rank owns gives VBX_E_INVALID and
+ * nothing changes: a replica never overwrites the copy of record.  Capacity errors as vbx_upload_blocks. */
+VBX_API int vbx_upload_blocks_device(vbx_ctx* ctx, int layer, const int32_t* d_idx3, uint64_t m,
+                                     const void* d_voxels, uint8_t updated_bits);
 /* Layer::removeBlock / removeAllBlocks (core/layer.h:163-164) */
 VBX_API int vbx_remove_blocks(vbx_ctx* ctx, int layer, const int32_t* idx3, uint64_t m);
 VBX_API int vbx_clear(vbx_ctx* ctx, int layer);
@@ -352,6 +369,9 @@ VBX_API int vbx_host_copy_ms(vbx_ctx* ctx, const void* src, size_t bytes, float*
 VBX_API int vbx_debug_sort(vbx_ctx* ctx, const void* keys, int key_bytes, uint32_t n, int key_bits, void* keys_out,
                    uint32_t* perm_out);
 VBX_API int vbx_debug_scan(vbx_ctx* ctx, const uint32_t* in, uint32_t n, uint32_t* out);
+/* Test hook: bytes of the page-locked staging buffer that vbx_mirror_updated / vbx_upload_blocks allocate on
+ * first use (0 while it has never been allocated). */
+VBX_API int vbx_debug_staging_bytes(const vbx_ctx* ctx, uint64_t* host_bytes);
 /* Diagnostic for the pipelined path (vbx_tsdf_integrate_async): with the environment variable
  * VBX_ASYNC_TIMELINE set before the first asynchronous submission, the hand-off events keep timestamps.
  * For each of the (at most cap_sets, 10 exist) hand-off sets: seq[k] = submission number of the last scan

@@ -28,6 +28,7 @@ assert TSDF_DTYPE.itemsize == 12 and ESDF_DTYPE.itemsize == 20
 
 LAYER_TSDF, LAYER_ESDF = 0, 1
 UPDATED_MAP, UPDATED_MESH, UPDATED_ESDF = 1, 2, 4  # Update::Status, core/block.h:15-18
+UPDATED_MIRROR = 8  # the engine's own "changed since it was last mirrored" mark (VBX_UPDATED_MIRROR)
 
 
 class TsdfIntegratorType:  # tsdf_integrator.h:30-41
@@ -137,7 +138,8 @@ EXPORTS = ["vbx_create", "vbx_destroy", "vbx_last_error", "vbx_version", "vbx_ge
            "vbx_host_alloc", "vbx_host_free", "vbx_host_copy_ms", "vbx_block_owner",
            "vbx_debug_sort", "vbx_debug_scan", "vbx_debug_bundle_order", "vbx_debug_apply", "vbx_debug_apply_paths", "vbx_debug_count_apply_paths", "vbx_debug_serial_fast", "vbx_debug_async_timeline", "vbx_tsdf_integrate_async", "vbx_esdf_update_blocks", "vbx_esdf_set_max_distance",
            "vbx_esdf_set_full_euclidean", "vbx_esdf_get_config", "vbx_esdf_add_robot_position", "vbx_esdf_clear", "vbx_mesh_generate", "vbx_mesh_download", "vbx_icp_run", "vbx_icp_run_device", "vbx_mirror_updated", "vbx_serialize_updated", "vbx_deserialize_blocks", "vbx_save_layer", "vbx_load_layer",
-           "vbx_proto_encode_layer", "vbx_proto_encode_block", "vbx_proto_decode_block"]
+           "vbx_proto_encode_layer", "vbx_proto_encode_block", "vbx_proto_decode_block",
+           "vbx_gather_updated_device", "vbx_upload_blocks_device", "vbx_debug_staging_bytes"]
 
 _lib = None
 
@@ -207,6 +209,12 @@ def load_library():
     lib.vbx_serialize_updated.argtypes = [vp, i32, i32, i32, vp, vp, vp, u64, C.POINTER(u64)]
     lib.vbx_deserialize_blocks.restype = i32
     lib.vbx_deserialize_blocks.argtypes = [vp, i32, vp, u64, vp, vp]
+    lib.vbx_gather_updated_device.argtypes = [vp, i32, i32, i32, i32, vp, vp, u64, C.POINTER(u64)]
+    lib.vbx_gather_updated_device.restype = i32
+    lib.vbx_upload_blocks_device.argtypes = [vp, i32, vp, u64, vp, C.c_uint8]
+    lib.vbx_upload_blocks_device.restype = i32
+    lib.vbx_debug_staging_bytes.restype = i32
+    lib.vbx_debug_staging_bytes.argtypes = [vp, C.POINTER(u64)]
     lib.vbx_save_layer.restype = i32
     lib.vbx_save_layer.argtypes = [vp, i32, C.c_char_p, i32]
     lib.vbx_load_layer.restype = i32
@@ -511,6 +519,44 @@ class Layer:
         ctx.check(ctx.lib.vbx_upload_blocks(ctx.handle, self._layer_id, idx.ctypes.data, idx.shape[0], vox.ctypes.data,
                                             None if upd is None else upd.ctypes.data), "vbx_upload_blocks")
 
+    def _block_bytes(self) -> int:
+        return (TSDF_DTYPE if self._layer_id == LAYER_TSDF else ESDF_DTYPE).itemsize * self._vps ** 3
+
+    def gatherUpdatedDevice(self, bit_mask: int = 0, clear_mask: int = 0, owned_only: bool = False,
+                            d_idx3=None, d_voxels=None, cap: Optional[int] = None) -> int:
+        """vbx_gather_updated_device: the blocks whose updated bits match `bit_mask` (0 = all; with owned_only
+        only the blocks this rank owns), ascending (x, y, z), gathered on the device into `d_idx3` (3 int32 per
+        block) and `d_voxels` (raw voxel payloads) -- CUDA tensors, or raw device pointers with `cap` -- and
+        `clear_mask` reset on them.  Returns the number of matching blocks; when it exceeds the capacity
+        (default: what both tensors hold, 0 without buffers) nothing is copied or cleared."""
+        ctx = self._bound()
+        if cap is None:
+            cap = 0 if d_idx3 is None else min(_nbytes(d_idx3) // 12, _nbytes(d_voxels) // self._block_bytes())
+        n = C.c_uint64(0)
+        ctx.check(ctx.lib.vbx_gather_updated_device(ctx.handle, self._layer_id, int(bit_mask), int(clear_mask),
+                                                    int(bool(owned_only)), _device_ptr(d_idx3), _device_ptr(d_voxels),
+                                                    int(cap), C.byref(n)), "vbx_gather_updated_device")
+        return int(n.value)
+
+    def insertBlocksDevice(self, d_idx3, d_voxels, m: Optional[int] = None,
+                           updated_bits: int = UPDATED_MAP | UPDATED_MESH | UPDATED_ESDF):
+        """vbx_upload_blocks_device: insertBlocks with the indices (m x 3 int32) and raw voxel payloads already on
+        the device (CUDA tensors, or raw device pointers with `m`); every written block's updated() bits become
+        `updated_bits` -- by default what Block::updated().set() gives a block a scan touched.  A sharded engine
+        refuses blocks its own rank owns."""
+        ctx = self._bound()
+        if m is None:
+            m = _nbytes(d_idx3) // 12
+        ctx.check(ctx.lib.vbx_upload_blocks_device(ctx.handle, self._layer_id, _device_ptr(d_idx3), int(m),
+                                                   _device_ptr(d_voxels), int(updated_bits)), "vbx_upload_blocks_device")
+
+    def stagingBytes(self) -> int:
+        """Bytes of the engine's page-locked staging buffer (0: never allocated; vbx_debug_staging_bytes)."""
+        ctx = self._bound()
+        n = C.c_uint64(0)
+        ctx.check(ctx.lib.vbx_debug_staging_bytes(ctx.handle, C.byref(n)), "vbx_debug_staging_bytes")
+        return int(n.value)
+
     def removeBlock(self, index: Sequence[int]):  # core/layer.h:163
         self.removeBlocks(np.asarray([index], dtype=np.int32))
 
@@ -528,6 +574,21 @@ class Layer:
         """block.updated().reset(bit) on every block (esdf_integrator.cc:113-121)."""
         ctx = self._bound()
         ctx.check(ctx.lib.vbx_clear_updated(ctx.handle, self._layer_id, 1 << bit), "vbx_clear_updated")
+
+
+def _device_ptr(x) -> Optional[int]:
+    """A CUDA tensor's (contiguous) data pointer, or a raw pointer as given."""
+    if x is None or isinstance(x, int):
+        return x
+    if not (x.is_cuda and x.is_contiguous()):
+        raise VoxbloxError("expected a contiguous CUDA tensor")
+    return x.data_ptr()
+
+
+def _nbytes(x) -> int:
+    if x is None or isinstance(x, int):
+        raise VoxbloxError("raw device pointers need an explicit size")
+    return x.numel() * x.element_size()
 
 
 def _as_pose(T_G_C) -> Tuple[np.ndarray, np.ndarray]:

@@ -120,7 +120,7 @@ __global__ void k_serialize_blocks(int layer, const uint32_t* __restrict__ pool,
 // contiguous payloads (raw voxel structs or block.cc words) -> pool slots; also the per-slot flags
 __global__ void k_scatter_blocks(int layer, int serialized, const uint32_t* __restrict__ in,
                                  const int32_t* __restrict__ slots, uint32_t m, uint32_t vox_per_block,
-                                 uint32_t* __restrict__ pool, const uint8_t* __restrict__ upd_in,
+                                 uint32_t* __restrict__ pool, const uint8_t* __restrict__ upd_in, uint8_t upd_all,
                                  uint8_t* __restrict__ flags, uint8_t* __restrict__ has_esdf) {
   const uint32_t b = blockIdx.y;
   if (b >= m) return;
@@ -142,7 +142,8 @@ __global__ void k_scatter_blocks(int layer, int serialized, const uint32_t* __re
     for (int k = 0; k < 5; ++k) dst[k] = v[k];
   }
   if (i == 0) {
-    flags[slot] = upd_in ? (uint8_t)(upd_in[b] & kReportedBits) : (uint8_t)0;  // (bit 7 is the engine's own; a TSDF upload clears kSlotNoTsdf)
+    // (bit 7 is the engine's own; a TSDF upload clears kSlotNoTsdf)
+    flags[slot] = (uint8_t)((upd_in ? upd_in[b] : upd_all) & kReportedBits);
     if (has_esdf) has_esdf[slot] = 1;
   }
 }
@@ -169,6 +170,73 @@ static size_t payload_bytes(const vbx_ctx* c, int layer, int serialized) {
   return (serialized ? 8u : sizeof(EsdfVoxel)) * c->vox_per_block;
 }
 
+// The packed keys of an upload's block indices; VBX_E_INVALID (before anything is written) for an index
+// outside +-2^20
+static int upload_keys(vbx_ctx* c, const int32_t* idx3, uint64_t m, std::vector<uint64_t>* keys) {
+  keys->resize(m);
+  for (uint64_t i = 0; i < m; ++i) {
+    const int32_t* p = idx3 + 3 * i;
+    const int lim = kCoordBias - 1;
+    if (p[0] < -lim || p[0] > lim || p[1] < -lim || p[1] > lim || p[2] < -lim || p[2] > lim) {
+      return fail(c, VBX_E_INVALID, "block index outside +-2^20");
+    }
+    (*keys)[i] = pack3(p[0], p[1], p[2]);
+  }
+  return VBX_OK;
+}
+
+// Find-or-create an upload's blocks.  Every block is created by k_assign, in rounds of at most as many keys as
+// hand-off set 0's table has ids (the point-key buffer holds the keys, the ray list their local ids); the slots
+// end in set 0's cnt.  *listed = the keys whose slots are known (a round that fails ends the listing), *err =
+// that round's state error (DESIGN.md section 9: the blocks created before the pool ran out stay).
+static int create_upload_blocks(vbx_ctx* c, int layer, const std::vector<uint64_t>& keys, uint64_t* listed, int* err) {
+  cudaStream_t s = c->stream;
+  const uint64_t m = keys.size();
+  const vbx_ctx::ScratchSet& S = c->set[0];
+  VBX_CUDA(c, cudaMemcpyAsync(S.pkeys0, keys.data(), m * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+  // a block inserted into the ESDF layer at an index the TSDF layer does not hold occupies a slot of its own
+  const uint8_t new_bits = layer == VBX_LAYER_ESDF ? kSlotNoTsdf : (uint8_t)0;
+  *err = VBX_OK;
+  *listed = 0;
+  while (*listed < m && *err == VBX_OK) {
+    const uint32_t rn = (uint32_t)std::min<uint64_t>(S.blocks.cap, m - *listed);
+    VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), s));
+    k_list_keys<<<grid_for(rn, 256), 256, 0, s>>>(S.blocks, S.pkeys0 + *listed, rn, S.ray_list + *listed, S.d_state);
+    if (int rc = create_listed_blocks(c, new_bits)) return rc;
+    k_slots_of<<<grid_for(rn, 256), 256, 0, s>>>(c->tab.hslot, S.touched_list, S.ray_list + *listed, rn,
+                                                  reinterpret_cast<int32_t*>(S.cnt) + *listed);
+    VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+    VBX_CUDA(c, cudaStreamSynchronize(s));
+    const ScanState& h = *S.h_state;
+    c->n_blocks = h.n_blocks;
+    if (layer == VBX_LAYER_ESDF && h.n_new) c->maybe_esdf_only = true;
+    *err = check_state_errors(c, h);
+    *listed += rn;
+  }
+  return VBX_OK;
+}
+
+// k_scatter_blocks of listed blocks [at, at + k) from the contiguous device payloads at `src`, in slices of
+// kMaxGridY blocks; the flags become d_upd[b] (device, per block) or, when d_upd is null, upd_all
+static int scatter_listed(vbx_ctx* c, int layer, int serialized, const void* src, uint64_t at, uint64_t k,
+                          const uint8_t* d_upd, uint8_t upd_all) {
+  const size_t bbytes = payload_bytes(c, layer, serialized);
+  const uint32_t wpv = (layer == VBX_LAYER_TSDF) ? 3u : (serialized ? 1u : 5u);  // threads per voxel along x
+  uint32_t* pool = layer == VBX_LAYER_TSDF ? reinterpret_cast<uint32_t*>(c->tab.tsdf) : reinterpret_cast<uint32_t*>(c->tab.esdf);
+  uint8_t* flags = layer == VBX_LAYER_TSDF ? c->tab.slot_updated : c->tab.slot_esdf_updated;
+  const int32_t* slots = reinterpret_cast<const int32_t*>(c->set[0].cnt) + at;
+  for (uint64_t b0 = 0; b0 < k; b0 += kMaxGridY) {
+    const uint64_t kb = std::min<uint64_t>(kMaxGridY, k - b0);
+    const dim3 grid(grid_for((uint64_t)wpv * c->vox_per_block, 256), (unsigned int)kb);
+    k_scatter_blocks<<<grid, 256, 0, c->stream>>>(
+        layer, serialized, reinterpret_cast<const uint32_t*>(static_cast<const char*>(src) + b0 * bbytes), slots + b0,
+        (uint32_t)kb, (uint32_t)c->vox_per_block, pool, d_upd ? d_upd + b0 : nullptr, upd_all, flags,
+        layer == VBX_LAYER_ESDF ? c->tab.slot_has_esdf : nullptr);
+    VBX_CUDA(c, cudaGetLastError());
+  }
+  return VBX_OK;
+}
+
 // Layer::insertBlock / allocateBlockPtrByIndex + voxel copy, or Block(BlockProto) + deserializeFromIntegers
 // (core/block_inl.h:73-109) when `serialized`: find-or-create the blocks, then ONE staged copy per
 // chunk and a scatter kernel.
@@ -178,45 +246,15 @@ int upload_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, const 
   if (layer == VBX_LAYER_ESDF && !c->has_esdf) return fail(c, VBX_E_STATE, "no ESDF layer");
   if (m > c->tab.max_blocks) return fail(c, VBX_E_CAPACITY, "more blocks than the pool holds");
   cudaStream_t s = c->stream;
-  std::vector<uint64_t> keys(m);
-  for (uint64_t i = 0; i < m; ++i) {
-    const int32_t* p = idx3 + 3 * i;
-    const int lim = kCoordBias - 1;
-    if (p[0] < -lim || p[0] > lim || p[1] < -lim || p[1] > lim || p[2] < -lim || p[2] > lim) {
-      return fail(c, VBX_E_INVALID, "block index outside +-2^20");
-    }
-    keys[i] = pack3(p[0], p[1], p[2]);
-  }
-  // scratch of hand-off set 0: the point-key buffer holds the keys, the ray list their local ids, cnt the slots
+  std::vector<uint64_t> keys;
+  if (int rc = upload_keys(c, idx3, m, &keys)) return rc;
   if (m > c->max_points) return fail(c, VBX_E_CAPACITY, "upload more than max_points_per_scan blocks at once");
-  const vbx_ctx::ScratchSet& S = c->set[0];
-  VBX_CUDA(c, cudaMemcpyAsync(S.pkeys0, keys.data(), m * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
-  // every block is created by k_assign, in rounds of at most as many keys as the table has ids; a block
-  // inserted into the ESDF layer at an index the TSDF layer does not hold occupies a slot of its own
-  const uint8_t new_bits = layer == VBX_LAYER_ESDF ? kSlotNoTsdf : (uint8_t)0;
+  uint64_t listed = 0;
   int err = VBX_OK;
-  uint64_t listed = 0;  // keys whose slots are known (a round that fails ends the listing)
-  while (listed < m && err == VBX_OK) {
-    const uint32_t rn = (uint32_t)std::min<uint64_t>(S.blocks.cap, m - listed);
-    VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), s));
-    k_list_keys<<<grid_for(rn, 256), 256, 0, s>>>(S.blocks, S.pkeys0 + listed, rn, S.ray_list + listed, S.d_state);
-    if (int rc = create_listed_blocks(c, new_bits)) return rc;
-    k_slots_of<<<grid_for(rn, 256), 256, 0, s>>>(c->tab.hslot, S.touched_list, S.ray_list + listed, rn,
-                                                  reinterpret_cast<int32_t*>(S.cnt) + listed);
-    VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
-    VBX_CUDA(c, cudaStreamSynchronize(s));
-    const ScanState& h = *S.h_state;
-    c->n_blocks = h.n_blocks;
-    if (layer == VBX_LAYER_ESDF && h.n_new) c->maybe_esdf_only = true;
-    err = check_state_errors(c, h);
-    listed += rn;
-  }
+  if (int rc = create_upload_blocks(c, layer, keys, &listed, &err)) return rc;
   // The payloads of the blocks that have slots, also when the pool ran out: every block the call created
   // holds what was uploaded for it (an ESDF block becomes one only here, by slot_has_esdf)
   const size_t bbytes = payload_bytes(c, layer, serialized);
-  const uint32_t wpv = (layer == VBX_LAYER_TSDF) ? 3u : (serialized ? 1u : 5u);  // threads per voxel along x
-  uint32_t* pool = layer == VBX_LAYER_TSDF ? reinterpret_cast<uint32_t*>(c->tab.tsdf) : reinterpret_cast<uint32_t*>(c->tab.esdf);
-  uint8_t* flags = layer == VBX_LAYER_TSDF ? c->tab.slot_updated : c->tab.slot_esdf_updated;
   const uint64_t chunk = std::max<uint64_t>(1, std::min<uint64_t>(listed, (256ull << 20) / bbytes));
   if (int rc = ensure_staging(c, chunk * bbytes + chunk, chunk)) return rc;
   uint8_t* d_upd = static_cast<uint8_t*>(c->mirror_dev) + chunk * bbytes;
@@ -225,17 +263,41 @@ int upload_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, const 
     VBX_CUDA(c, cudaMemcpyAsync(c->mirror_dev, static_cast<const char*>(voxels) + at * bbytes, k * bbytes,
                                 cudaMemcpyHostToDevice, s));
     if (updated_bits) VBX_CUDA(c, cudaMemcpyAsync(d_upd, updated_bits + at, k, cudaMemcpyHostToDevice, s));
-    for (uint64_t b0 = 0; b0 < k; b0 += kMaxGridY) {
-      const uint64_t kb = std::min<uint64_t>(kMaxGridY, k - b0);
-      const dim3 grid(grid_for((uint64_t)wpv * c->vox_per_block, 256), (unsigned int)kb);
-      k_scatter_blocks<<<grid, 256, 0, s>>>(
-          layer, serialized, reinterpret_cast<const uint32_t*>(static_cast<const char*>(c->mirror_dev) + b0 * bbytes),
-          reinterpret_cast<const int32_t*>(S.cnt) + at + b0, (uint32_t)kb, (uint32_t)c->vox_per_block, pool,
-          updated_bits ? d_upd + b0 : nullptr, flags, layer == VBX_LAYER_ESDF ? c->tab.slot_has_esdf : nullptr);
-      VBX_CUDA(c, cudaGetLastError());
-    }
+    if (int rc = scatter_listed(c, layer, serialized, c->mirror_dev, at, k, updated_bits ? d_upd : nullptr, 0)) return rc;
     VBX_CUDA(c, cudaStreamSynchronize(s));  // the staging buffer is reused by the next chunk
   }
+  if (err) return err;
+  return refresh_host_mirror(c);
+}
+
+// upload_blocks with the raw voxel payloads already in device memory: the blocks are created the same way and
+// scattered straight from `d_voxels`, every written slot's flags set to `updated_bits` (reported bits only).
+// k_list_keys takes packed keys, and the range and ownership checks must pass before anything is written, so
+// the indices (12 B per block, never a payload byte) are read to the host once.  On a sharded engine a block
+// this rank owns is refused: its copy of record is the one the integrators update here.
+int upload_blocks_device(vbx_ctx* c, int layer, const int32_t* d_idx3, uint64_t m, const void* d_voxels,
+                         uint8_t updated_bits) {
+  if (m == 0) return VBX_OK;
+  if (layer == VBX_LAYER_ESDF && !c->has_esdf) return fail(c, VBX_E_STATE, "no ESDF layer");
+  if (m > c->tab.max_blocks) return fail(c, VBX_E_CAPACITY, "more blocks than the pool holds");
+  std::vector<int32_t> idx(3 * m);
+  VBX_CUDA(c, cudaMemcpyAsync(idx.data(), d_idx3, 3 * m * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  VBX_CUDA(c, cudaStreamSynchronize(c->stream));
+  std::vector<uint64_t> keys;
+  if (int rc = upload_keys(c, idx.data(), m, &keys)) return rc;
+  if (c->opt.world_size > 1) {
+    for (uint64_t i = 0; i < m; ++i) {
+      if (block_owner(idx[3 * i], idx[3 * i + 1], idx[3 * i + 2], c->opt.world_size) == c->opt.rank) {
+        return fail(c, VBX_E_INVALID, "a replica upload names a block this rank owns");
+      }
+    }
+  }
+  if (m > c->max_points) return fail(c, VBX_E_CAPACITY, "upload more than max_points_per_scan blocks at once");
+  uint64_t listed = 0;
+  int err = VBX_OK;
+  if (int rc = create_upload_blocks(c, layer, keys, &listed, &err)) return rc;
+  if (int rc = scatter_listed(c, layer, 0, d_voxels, 0, listed, nullptr, updated_bits)) return rc;
+  VBX_CUDA(c, cudaStreamSynchronize(c->stream));
   if (err) return err;
   return refresh_host_mirror(c);
 }
@@ -526,6 +588,65 @@ int mirror_updated(vbx_ctx* c, int layer, int updated_mask, int clear_mask, int3
   VBX_CUDA(c, cudaStreamSynchronize(s));
   VBX_CUDA(c, cudaGetLastError());
   if (!direct && voxels) std::memcpy(voxels, c->mirror_host, m * bbytes);
+  return VBX_OK;
+}
+
+// The gather half of mirror_updated into caller-owned device memory (the payloads of one GPU's blocks handed
+// to another GPU).  The ownership filter and the (x, y, z) order are taken on the host view of the slots: it is
+// one flag byte per block that every layer call reads anyway, and the keys are already in the host mirror,
+// whereas a device compaction would need a device sort to give the same order.  The indices travel host ->
+// device; only the flag bytes come back, never a payload byte.
+int gather_updated_device(vbx_ctx* c, int layer, int updated_mask, int clear_mask, int owned_only, int32_t* d_idx3,
+                          void* d_voxels, uint64_t cap, uint64_t* n) {
+  cudaStream_t s = c->stream;
+  *n = 0;
+  if (c->n_blocks == 0) return VBX_OK;
+  LayerSlots view;
+  if (int rc = read_layer_slots(c, layer, &view)) return rc;
+  std::vector<LayerSlots::Entry> items = view.sorted(kMirrorBits, updated_mask);
+  if (owned_only && c->opt.world_size > 1) {
+    const int w = c->opt.world_size, r = c->opt.rank;
+    items.erase(std::remove_if(items.begin(), items.end(),
+                               [&](const LayerSlots::Entry& e) { return block_owner(e.x, e.y, e.z, w) != r; }),
+                items.end());
+  }
+  *n = items.size();
+  if (items.empty() || items.size() > cap) return VBX_OK;  // (too small a buffer: nothing copied or cleared)
+  const size_t m = items.size();
+  if (m > c->xfer_cap_slots) {
+    if (c->xfer_slots) cudaFree(c->xfer_slots);
+    c->xfer_slots = nullptr;
+    c->xfer_cap_slots = 0;
+    const size_t want = std::max<size_t>(2 * m, 1024);
+    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->xfer_slots), want * sizeof(uint32_t)));
+    c->xfer_cap_slots = want;
+  }
+  std::vector<int32_t> idx(3 * m);
+  std::vector<uint32_t> slots(m);
+  for (size_t i = 0; i < m; ++i) {
+    slots[i] = items[i].slot;
+    idx[3 * i] = items[i].x;
+    idx[3 * i + 1] = items[i].y;
+    idx[3 * i + 2] = items[i].z;
+  }
+  VBX_CUDA(c, cudaMemcpyAsync(d_idx3, idx.data(), 3 * m * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  VBX_CUDA(c, cudaMemcpyAsync(c->xfer_slots, slots.data(), m * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+  uint8_t* flags = (layer == VBX_LAYER_TSDF) ? c->tab.slot_updated : c->tab.slot_esdf_updated;
+  const size_t raw_bytes = ((layer == VBX_LAYER_TSDF) ? sizeof(TsdfVoxel) : sizeof(EsdfVoxel)) * c->vox_per_block;
+  const char* pool = (layer == VBX_LAYER_TSDF) ? reinterpret_cast<const char*>(c->tab.tsdf)
+                                               : reinterpret_cast<const char*>(c->tab.esdf);
+  const uint8_t clear = (uint8_t)(clear_mask & kMirrorBits);
+  if (raw_bytes % 16 == 0 && reinterpret_cast<uintptr_t>(d_voxels) % 16 == 0) {
+    k_gather_blocks<<<(unsigned int)(m * 8), 256, 0, s>>>(reinterpret_cast<const uint4*>(pool), c->xfer_slots,
+                                                           (uint32_t)m, (uint32_t)(raw_bytes / 16),
+                                                           static_cast<uint4*>(d_voxels), flags, clear);
+  } else {
+    k_gather_words<<<grid_for((uint64_t)m * (raw_bytes / 4), 256), 256, 0, s>>>(
+        reinterpret_cast<const uint32_t*>(pool), c->xfer_slots, (uint32_t)m, (uint32_t)(raw_bytes / 4),
+        static_cast<uint32_t*>(d_voxels), flags, clear);
+  }
+  VBX_CUDA(c, cudaGetLastError());
+  VBX_CUDA(c, cudaStreamSynchronize(s));  // (idx and slots live on this stack frame)
   return VBX_OK;
 }
 

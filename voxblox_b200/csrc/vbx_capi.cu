@@ -468,6 +468,7 @@ void vbx_destroy(vbx_ctx* c) {
   if (c->mirror_dev) cudaFree(c->mirror_dev);
   if (c->mirror_host) cudaFreeHost(c->mirror_host);
   if (c->mirror_slots) cudaFree(c->mirror_slots);
+  if (c->xfer_slots) cudaFree(c->xfer_slots);
   for (vbx_ctx::ScratchSet& S : c->set) free_set(S);
   for (vbx_ctx::FrontLane& F : c->lane) free_lane(F);
   if (c->timeline_ref) cudaEventDestroy(c->timeline_ref);
@@ -800,6 +801,46 @@ int vbx_upload_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, co
   VBX_CUDA(c, cudaSetDevice(c->device));
   VBX_DRAIN(c);
   return upload_blocks(c, layer, idx3, m, voxels, updated_bits, 0);
+}
+
+// device memory of this process (cudaMalloc, or managed), 4-byte aligned: the transfer kernels read and write
+// 32-bit words
+static bool device_words(const void* p) {
+  cudaPointerAttributes a;
+  const bool dev = cudaPointerGetAttributes(&a, p) == cudaSuccess &&
+                   (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged);
+  cudaGetLastError();  // (an unregistered host pointer may leave an error code behind)
+  return dev && reinterpret_cast<uintptr_t>(p) % 4 == 0;
+}
+
+int vbx_gather_updated_device(vbx_ctx* c, int layer, int updated_mask, int clear_mask, int owned_only, int32_t* d_idx3,
+                              void* d_voxels, uint64_t cap, uint64_t* n) {
+  if (!c || !n || (cap && (!d_idx3 || !d_voxels))) return fail(c, VBX_E_INVALID, "null argument");
+  VBX_CUDA(c, cudaSetDevice(c->device));
+  if (cap && (!device_words(d_idx3) || !device_words(d_voxels))) {
+    return fail(c, VBX_E_INVALID, "d_idx3 / d_voxels must be 4-byte aligned device memory");
+  }
+  VBX_DRAIN(c);
+  *n = 0;
+  if (layer == VBX_LAYER_ESDF && !c->has_esdf) return VBX_OK;
+  return gather_updated_device(c, layer, updated_mask, clear_mask, owned_only, d_idx3, d_voxels, cap, n);
+}
+
+int vbx_upload_blocks_device(vbx_ctx* c, int layer, const int32_t* d_idx3, uint64_t m, const void* d_voxels,
+                             uint8_t updated_bits) {
+  if (!c || (m && (!d_idx3 || !d_voxels))) return fail(c, VBX_E_INVALID, "null argument");
+  VBX_CUDA(c, cudaSetDevice(c->device));
+  if (m && (!device_words(d_idx3) || !device_words(d_voxels))) {
+    return fail(c, VBX_E_INVALID, "d_idx3 / d_voxels must be 4-byte aligned device memory");
+  }
+  VBX_DRAIN(c);
+  return upload_blocks_device(c, layer, d_idx3, m, d_voxels, updated_bits);
+}
+
+int vbx_debug_staging_bytes(const vbx_ctx* c, uint64_t* host_bytes) {
+  if (!c || !host_bytes) return VBX_E_INVALID;
+  *host_bytes = c->mirror_host ? c->mirror_cap_bytes : 0;
+  return VBX_OK;
 }
 
 int vbx_remove_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m) {

@@ -325,6 +325,9 @@ struct vbx_ctx {
   void* mirror_host = nullptr;  // page-locked
   uint32_t* mirror_slots = nullptr;
   size_t mirror_cap_bytes = 0, mirror_cap_slots = 0;
+  // device-to-device block transfer (vbx_gather_updated_device): the gathered blocks' slots, device only
+  uint32_t* xfer_slots = nullptr;
+  size_t xfer_cap_slots = 0;
   // host mirror of slot_key (refreshed lazily)
   std::vector<uint64_t> host_slot_key;
   std::unordered_map<uint64_t, int32_t> host_key2slot;
@@ -414,6 +417,10 @@ int read_layer_slots(vbx_ctx* c, int layer, LayerSlots* view);
 int keep_flag_bits(vbx_ctx* c, uint8_t* flags, uint8_t keep);
 int mirror_updated(vbx_ctx* c, int layer, int updated_mask, int clear_mask, int32_t* idx3, void* voxels,
                    uint8_t* updated_bits, uint64_t cap, uint64_t* n, int serialized);
+int gather_updated_device(vbx_ctx* c, int layer, int updated_mask, int clear_mask, int owned_only, int32_t* d_idx3,
+                          void* d_voxels, uint64_t cap, uint64_t* n);
+int upload_blocks_device(vbx_ctx* c, int layer, const int32_t* d_idx3, uint64_t m, const void* d_voxels,
+                         uint8_t updated_bits);
 int esdf_destroy(vbx_ctx* c);
 void mesh_destroy(vbx_ctx* c);
 void icp_destroy(vbx_ctx* c);

@@ -15,16 +15,24 @@ from different ray ranges cannot be combined into the reference's result.  Owner
 every voxel's update chain on one GPU instead.
 
 This module holds the host-side logic: the ownership function (mirrors vbx_block_owner), gathering
-the shards into one block dictionary, and keeping read-only replicas of the other ranks' dirty blocks
-(`sync_replicas`, one all-gather of the blocks dirtied since the last call).
+the shards into one block dictionary, and keeping read-only replicas of the other ranks' dirty blocks:
+`exchange` moves them GPU to GPU (device gather, one all-gather of CUDA tensors, device upload), so
+that the ESDF, the mesher and ICP of every rank see the whole map; `sync_replicas` is the older path
+through host memory.
 """
 from __future__ import annotations
 
-from typing import Dict, Optional, Tuple
+import threading
+from typing import Callable, Dict, Optional, Tuple
 
 import numpy as np
 
-from .api import EngineOptions, Layer, VoxbloxError
+from .api import (UPDATED_ESDF, UPDATED_MAP, UPDATED_MESH, UPDATED_MIRROR, EngineOptions, Layer,
+                  VoxbloxError)
+
+# the updated() bits a replica carries: what Block::updated().set() gives a block a scan touched
+# (tsdf_integrator.cc:91-134), so incremental consumers on the receiving rank see it as the owner's would
+REPLICA_BITS = UPDATED_MAP | UPDATED_MESH | UPDATED_ESDF
 
 
 # ------------------------------------------------------------------ host logic (CPU-testable)
@@ -84,18 +92,57 @@ def all_gather_blocks(indices: np.ndarray, voxels: np.ndarray, group=None):
     return np.concatenate(out_idx), np.concatenate(out_vox), counts
 
 
+def nccl_all_gather(group=None) -> Callable:
+    """all_gather(out, inp): torch.distributed.all_gather_into_tensor over `group` (NCCL on CUDA tensors)."""
+    import torch.distributed as dist
+
+    return lambda out, inp: dist.all_gather_into_tensor(out, inp, group=group)
+
+
+class LocalAllGather:
+    """The all-gather of W ranks that are W threads of one process, each with its own engine (all on one
+    GPU, or several): rank r calls `gather.rank(r)(out, inp)` from its thread, as it would call
+    all_gather_into_tensor.  Lets a sharded map run without torch.distributed (tests, single-GPU
+    measurement)."""
+
+    def __init__(self, world: int, timeout: float = 300.0):
+        self.world = world
+        self._inputs = [None] * world
+        self._barrier = threading.Barrier(world, timeout=timeout)
+
+    def rank(self, r: int) -> Callable:
+        import torch
+
+        def gather(out, inp):
+            self._inputs[r] = inp
+            self._barrier.wait()
+            torch.cat([p.to(out.device) for p in self._inputs], out=out)
+            self._barrier.wait()  # (no rank replaces its input before every rank has read it)
+
+        return gather
+
+
 class ShardedLayer:
     """The block-sharded map as its callers see it.
 
-    `layer` is this rank's shard (a Layer whose engine was created with shard_options)."""
+    `layer` is this rank's shard (a Layer whose engine was created with shard_options).  `all_gather`
+    (out, inp) is the collective exchange() uses, all_gather_into_tensor over `group` by default; with
+    another one (LocalAllGather) rank and world come from the layer's engine options."""
 
-    def __init__(self, layer: Layer, group=None):
-        import torch.distributed as dist
-
+    def __init__(self, layer: Layer, group=None, all_gather: Optional[Callable] = None):
         self.layer = layer
         self.group = group
-        self.rank = dist.get_rank(group)
-        self.world = dist.get_world_size(group)
+        if all_gather is None:
+            import torch.distributed as dist
+
+            self.rank = dist.get_rank(group)
+            self.world = dist.get_world_size(group)
+            all_gather = nccl_all_gather(group)
+        else:
+            self.rank = int(layer.engine_options.rank)
+            self.world = int(layer.engine_options.world_size)
+        self.all_gather = all_gather
+        self.last_exchange: Dict[str, int] = {}
 
     def owned(self, indices) -> np.ndarray:
         return block_owner(indices, self.world) == self.rank
@@ -128,3 +175,49 @@ class ShardedLayer:
             self.layer.insertBlocks(all_idx[theirs], all_vox[theirs].view(vox.dtype).reshape(int(theirs.sum()), -1),
                                     updated_bits=np.zeros(int(theirs.sum()), np.uint8))
         return int(theirs.sum())
+
+    def exchange(self, layer: Optional[Layer] = None) -> int:
+        """Bring every rank's read-only replicas of the other ranks' blocks up to date, GPU to GPU.
+
+        1. The blocks this rank owns that changed since the last exchange (the engine's own
+           VBX_UPDATED_MIRROR mark, cleared here; the owner's kMap / kMesh / kEsdf bits stay with its own
+           consumers) are gathered on the device into one padded CUDA buffer.
+        2. One all-gather of the counts, one all-gather of the indices and payloads.
+        3. The other ranks' blocks are written into this rank's map with REPLICA_BITS set.
+        Afterwards every rank holds the whole map as of the last scan.  Block removals do not propagate:
+        the caller removes a block on every rank.  `layer` defaults to the TSDF shard (an ESDF Layer of the
+        same engine may be passed).  Returns the number of blocks received; `last_exchange` holds the
+        counts and bytes of the call."""
+        import torch
+
+        lay = self.layer if layer is None else layer
+        opt = lay.engine_options
+        dev = torch.device("cuda", opt.device if opt is not None and opt.device >= 0 else torch.cuda.current_device())
+        bb = lay._block_bytes()
+        n = lay.gatherUpdatedDevice(UPDATED_MIRROR, owned_only=True)  # the count only (cap 0: nothing cleared)
+        counts = torch.zeros(self.world, dtype=torch.int64, device=dev)
+        self.all_gather(counts, torch.full((1,), n, dtype=torch.int64, device=dev))
+        counts = counts.tolist()
+        cap = int(max(counts))
+        self.last_exchange = dict(sent=n, received=0, bytes=0)
+        if cap == 0:
+            return 0
+        # one buffer per rank: cap payloads (16-byte aligned for the gather's vector stores), then cap indices
+        per = cap * (bb + 12)
+        send = torch.empty(per, dtype=torch.uint8, device=dev)
+        if lay.gatherUpdatedDevice(UPDATED_MIRROR, clear_mask=UPDATED_MIRROR, owned_only=True,
+                                   d_idx3=send[cap * bb:cap * bb + 12 * n], d_voxels=send[:n * bb], cap=n) != n:
+            raise VoxbloxError("the owned dirty blocks changed between the count and the gather")
+        recv = torch.empty(self.world * per, dtype=torch.uint8, device=dev)
+        self.all_gather(recv, send)
+        torch.cuda.current_stream(dev).synchronize()  # (the engine reads recv on its own stream)
+        got = 0
+        for r, c in enumerate(counts):
+            if r == self.rank or c == 0:
+                continue
+            base = r * per
+            lay.insertBlocksDevice(recv[base + cap * bb:base + cap * bb + 12 * c], recv[base:base + c * bb], m=c,
+                                   updated_bits=REPLICA_BITS)
+            got += c
+        self.last_exchange = dict(sent=n, received=got, bytes=got * (bb + 12))
+        return got
