@@ -369,6 +369,16 @@ VBX_API int vbx_host_copy_ms(vbx_ctx* ctx, const void* src, size_t bytes, float*
 VBX_API int vbx_debug_sort(vbx_ctx* ctx, const void* keys, int key_bytes, uint32_t n, int key_bits, void* keys_out,
                    uint32_t* perm_out);
 VBX_API int vbx_debug_scan(vbx_ctx* ctx, const uint32_t* in, uint32_t n, uint32_t* out);
+/* Test hook for ICP's per-batch arithmetic (the functions vbx_icp_run applies to each mini batch), one
+ * device thread per item i < n, row-major 3 x 3 matrices and (w, x, y, z) quaternions:
+ *   r_out[9i ..]    the batch rotation of the cross-covariance h[9i ..] (2-D closed form when
+ *                   refine_roll_pitch == 0, 3-D SVD otherwise), valid_out[i] = 1 when ICP would fuse it
+ *                   (finite and a valid rotation matrix), else 0;
+ *   q_out[4i ..]    the quaternion of the rotation matrix m[9i ..];
+ *   log_out[3i ..]  the SO(3) log of the quaternion q[4i ..];  exp_out[4i ..] the exp of the vector w[3i ..]. */
+VBX_API int vbx_debug_icp_solve(vbx_ctx* ctx, uint32_t n, int refine_roll_pitch, const float* h, const float* m,
+                                const float* q, const float* w, float* r_out, int32_t* valid_out, float* q_out,
+                                float* log_out, float* exp_out);
 /* Test hook: bytes of the page-locked staging buffer that vbx_mirror_updated / vbx_upload_blocks allocate on
  * first use (0 while it has never been allocated). */
 VBX_API int vbx_debug_staging_bytes(const vbx_ctx* ctx, uint64_t* host_bytes);

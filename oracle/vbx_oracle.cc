@@ -1417,9 +1417,11 @@ inline bool rotationFromH3(const float hf[3][3], float r[3][3]) {
     sv[c] = std::sqrt(b[order[c]][order[c]] > 0 ? b[order[c]][order[c]] : 0.0);
     for (int k = 0; k < 3; ++k) vs[k][c] = v[k][order[c]];
   }
+  // sqrt of an eigenvalue of H^T H is a relative 1e-16 (s1 / s_c)^2 off: below 1e-4 s1, H v_c / s_c is no
+  // longer orthonormal to float accuracy (a planar batch leaves s3 ~ 1e-8 s1 of noise), so complete instead
   int good = 0;
   for (int c = 0; c < 3; ++c) {
-    if (sv[c] > 1e-12 * (sv[0] > 0 ? sv[0] : 1.0) && sv[c] > 0) {
+    if (sv[c] > 1e-4 * sv[0] && sv[c] > 0) {
       for (int i = 0; i < 3; ++i) {
         double s = 0;
         for (int k = 0; k < 3; ++k) s += a[i][k] * vs[k][c];
@@ -1430,16 +1432,18 @@ inline bool rotationFromH3(const float hf[3][3], float r[3][3]) {
       break;
     }
   }
+  // completion: H v_c, else the first unit vector left, made orthogonal to the columns before it
   for (int c = good; c < 3; ++c)
-    for (int e = 0; e < 3; ++e) {
-      double w[3] = {e == 0 ? 1.0 : 0.0, e == 1 ? 1.0 : 0.0, e == 2 ? 1.0 : 0.0};
+    for (int e = -1; e < 3; ++e) {
+      double w[3];
+      for (int i = 0; i < 3; ++i) w[i] = e < 0 ? a[i][0] * vs[0][c] + a[i][1] * vs[1][c] + a[i][2] * vs[2][c] : (i == e ? 1.0 : 0.0);
       for (int p = 0; p < c; ++p) {
         double dp = 0;
         for (int i = 0; i < 3; ++i) dp += w[i] * u[i][p];
         for (int i = 0; i < 3; ++i) w[i] -= dp * u[i][p];
       }
       const double nn = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
-      if (nn > 0.1) {
+      if (nn > (e < 0 ? 1e-24 * sv[0] * sv[0] : 0.1)) {
         for (int i = 0; i < 3; ++i) u[i][c] = w[i] / std::sqrt(nn);
         break;
       }
@@ -1458,6 +1462,18 @@ inline bool rotationFromH3(const float hf[3][3], float r[3][3]) {
     for (int i = 0; i < 3; ++i) vf[i][2] = vf[i][2] * -1.0f;
   for (int i = 0; i < 3; ++i)
     for (int j = 0; j < 3; ++j) r[i][j] = vf[i][0] * uf[j][0] + vf[i][1] * uf[j][1] + vf[i][2] * uf[j][2];
+  return true;
+}
+
+// minkindr's Rotation::isValidRotationMatrix with the threshold of oracle/shim/kindr (1000 float epsilons)
+inline bool isValidRotation(const float m[3][3]) {
+  const float thr = 1000.0f * std::numeric_limits<float>::epsilon();
+  const float det = m[0][0] * (m[1][1] * m[2][2] - m[1][2] * m[2][1]) - m[0][1] * (m[1][0] * m[2][2] - m[1][2] * m[2][0]) +
+                    m[0][2] * (m[1][0] * m[2][1] - m[1][1] * m[2][0]);
+  if (std::fabs(det - 1.0f) > thr) return false;
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j)
+      if (std::fabs(m[i][0] * m[j][0] + m[i][1] * m[j][1] + m[i][2] * m[j][2] - (i == j ? 1.0f : 0.0f)) > thr) return false;
   return true;
 }
 
@@ -1570,7 +1586,7 @@ struct IcpRunner {
       // the proper rotation V diag(1, det) U^T of the 2 x 2 SVD maximises trace(R H): closed form
       const float a = h[0][0] + h[1][1], b = h[0][1] - h[1][0];
       const float nrm = std::sqrt(a * a + b * b);
-      const float c = a / nrm, s = b / nrm;
+      const float c = nrm == 0.0f ? 1.0f : a / nrm, s = nrm == 0.0f ? 0.0f : b / nrm;  // H = 0: SVD U = V = I
       r[0][0] = c;
       r[0][1] = -s;
       r[1][0] = s;
@@ -1581,7 +1597,7 @@ struct IcpRunner {
     float sum = 0;
     for (int i = 0; i < 3; ++i)
       for (int j = 0; j < 3; ++j) sum += r[i][j];
-    if (!std::isfinite(sum)) return out;
+    if (!std::isfinite(sum) || !isValidRotation(r)) return out;  // icp.h:183-189
     out.delta.q = quatFromMatrix(r);
     out.delta.t = tc - qrot(out.delta.q, sc);
     out.ok = true;

@@ -22,6 +22,7 @@ from tests import test_esdf_options_gpu as teo  # noqa: E402
 from tests import test_esdf_reference_gpu as te  # noqa: E402
 from tests import test_fast_reference_gpu as tf  # noqa: E402
 from tests import test_icp_cpu as tic  # noqa: E402
+from tests import test_icp_degenerate_gpu as tid  # noqa: E402
 from tests import test_icp_gpu as ti  # noqa: E402
 from tests import test_merged_reference_gpu as tm  # noqa: E402
 from tests import test_mesh_cpu as tmc  # noqa: E402
@@ -57,6 +58,8 @@ def cases():
         out[f"tsdf_ground_truth/{key}"] = lambda lib, k=key: tg.reference_side(k, lib)[1]
     for key in ti.PIN_KEYS:
         out[f"icp/{key}"] = lambda lib, k=key: ti.reference_side(k, lib)[2]
+    for key in tid.PIN_KEYS:
+        out[f"icp_degenerate/{key}"] = lambda lib, k=key: tid.reference_side(k, lib)[1]
     for key in tb.PIN_KEYS:
         out[f"block_sizes/{key}"] = lambda lib, k=key: tb.reference_side(k, lib)[2]
     for key in tf.PIN_KEYS:
@@ -74,7 +77,7 @@ def main(prefixes=()):
         if prefixes and not key.startswith(tuple(prefixes)):
             continue
         pinned[key] = fn(ref)
-        if key.startswith("icp/refine") or key.startswith("block_sizes/icp/"):
+        if key.startswith(("icp/refine", "icp_degenerate/", "block_sizes/icp/")):
             same = fn(port)["map"] == pinned[key]["map"]   # the restatement's ICP is compared at 1e-5, not bit for bit
         elif key == "mesh/mc_tables":
             same = True                                     # the restatement owns no copy of the table

@@ -139,7 +139,8 @@ EXPORTS = ["vbx_create", "vbx_destroy", "vbx_last_error", "vbx_version", "vbx_ge
            "vbx_debug_sort", "vbx_debug_scan", "vbx_debug_bundle_order", "vbx_debug_apply", "vbx_debug_apply_paths", "vbx_debug_count_apply_paths", "vbx_debug_serial_fast", "vbx_debug_async_timeline", "vbx_tsdf_integrate_async", "vbx_esdf_update_blocks", "vbx_esdf_set_max_distance",
            "vbx_esdf_set_full_euclidean", "vbx_esdf_get_config", "vbx_esdf_add_robot_position", "vbx_esdf_clear", "vbx_mesh_generate", "vbx_mesh_download", "vbx_icp_run", "vbx_icp_run_device", "vbx_mirror_updated", "vbx_serialize_updated", "vbx_deserialize_blocks", "vbx_save_layer", "vbx_load_layer",
            "vbx_proto_encode_layer", "vbx_proto_encode_block", "vbx_proto_decode_block",
-           "vbx_gather_updated_device", "vbx_upload_blocks_device", "vbx_debug_staging_bytes"]
+           "vbx_gather_updated_device", "vbx_upload_blocks_device", "vbx_debug_staging_bytes",
+           "vbx_debug_icp_solve"]
 
 _lib = None
 
@@ -215,6 +216,8 @@ def load_library():
     lib.vbx_upload_blocks_device.restype = i32
     lib.vbx_debug_staging_bytes.restype = i32
     lib.vbx_debug_staging_bytes.argtypes = [vp, C.POINTER(u64)]
+    lib.vbx_debug_icp_solve.restype = i32
+    lib.vbx_debug_icp_solve.argtypes = [vp, C.c_uint32, i32] + [vp] * 9
     lib.vbx_save_layer.restype = i32
     lib.vbx_save_layer.argtypes = [vp, i32, C.c_char_p, i32]
     lib.vbx_load_layer.restype = i32

@@ -904,6 +904,15 @@ int vbx_icp_run_device(vbx_ctx* c, const vbx_icp_config* cfg, const float* d_poi
   return icp_run(c, cfg, d_points_C, 1, n, q_wxyz, t, seed, out_q_wxyz, out_t, num_updates);
 }
 
+int vbx_debug_icp_solve(vbx_ctx* c, uint32_t n, int refine_roll_pitch, const float* h, const float* m, const float* q,
+                        const float* w, float* r_out, int32_t* valid_out, float* q_out, float* log_out, float* exp_out) {
+  if (!c || (n && (!h || !m || !q || !w || !r_out || !valid_out || !q_out || !log_out || !exp_out)))
+    return fail(c, VBX_E_INVALID, "null argument");
+  VBX_CUDA(c, cudaSetDevice(c->device));
+  VBX_DRAIN(c);
+  return icp_debug_solve(c, n, refine_roll_pitch, h, m, q, w, r_out, valid_out, q_out, log_out, exp_out);
+}
+
 int vbx_mesh_download(vbx_ctx* c, int32_t* idx3, uint64_t* first_vertex, float* vertices, float* normals,
                       uint8_t* colors) {
   if (!c) return VBX_E_INVALID;

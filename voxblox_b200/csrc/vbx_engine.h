@@ -424,6 +424,8 @@ int upload_blocks_device(vbx_ctx* c, int layer, const int32_t* d_idx3, uint64_t 
 int esdf_destroy(vbx_ctx* c);
 void mesh_destroy(vbx_ctx* c);
 void icp_destroy(vbx_ctx* c);
+int icp_debug_solve(vbx_ctx* c, uint32_t n, int refine_roll_pitch, const float* h, const float* m, const float* q,
+                    const float* w, float* r_out, int32_t* valid_out, float* q_out, float* log_out, float* exp_out);
 int icp_run(vbx_ctx* c, const vbx_icp_config* cfg, const float* points, int on_device, uint64_t n, const float q[4],
             const float t[3], uint32_t seed, float out_q[4], float out_t[3], uint64_t* num_updates);
 int mesh_generate(vbx_ctx* c, const vbx_mesh_config* cfg, int only_updated, int clear_flag, uint64_t* n_blocks_out,

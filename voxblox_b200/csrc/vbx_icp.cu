@@ -21,7 +21,7 @@
 // Arithmetic: float32 with one rounding per operation (the library is built with -fmad=false), in the
 // operation order of the reference's Eigen / minkindr expressions.  The 2-D
 // Procrustes rotation (refine_roll_pitch = false) uses the closed form atan2(h01 - h10, h00 + h11) of
-// V diag(1, det) U^T; the 3-D one an SVD by Jacobi rotations on H^T H in double.
+// V diag(1, det) U^T; the 3-D one an SVD by Jacobi rotations on H^T H in double (vbx_icp_math.cuh).
 #include <algorithm>
 #include <cmath>
 #include <limits>
@@ -31,6 +31,7 @@
 
 #include "vbx_engine.h"
 #include "vbx_hash.cuh"
+#include "vbx_icp_math.cuh"
 #include "vbx_math.cuh"
 
 namespace vbx {
@@ -46,201 +47,6 @@ struct IcpParams {
   float eps4_f;   // epsilon^(1/4), float
   double eps4_d;  // epsilon^(1/4), double
 };
-
-struct IcpQuat {
-  float w, x, y, z;
-};
-struct IcpSE3 {
-  IcpQuat q;
-  F3 t;
-};
-
-__device__ __forceinline__ IcpQuat icp_qmul(const IcpQuat& a, const IcpQuat& b) {
-  IcpQuat r;
-  r.w = a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z;
-  r.x = a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y;
-  r.y = a.w * b.y + a.y * b.w + a.z * b.x - a.x * b.z;
-  r.z = a.w * b.z + a.z * b.w + a.x * b.y - a.y * b.x;
-  return r;
-}
-__device__ __forceinline__ F3 icp_qrot(const IcpQuat& q, F3 p) {
-  const F3 qv = f3(q.x, q.y, q.z);
-  F3 uv = cross3(qv, p);
-  uv = add3(uv, uv);
-  return add3(add3(p, scale3(uv, q.w)), cross3(qv, uv));
-}
-__device__ __forceinline__ IcpSE3 icp_mul(const IcpSE3& a, const IcpSE3& b) {
-  IcpSE3 r;
-  r.q = icp_qmul(a.q, b.q);
-  r.t = add3(a.t, icp_qrot(a.q, b.t));
-  return r;
-}
-__device__ __forceinline__ IcpSE3 icp_inv(const IcpSE3& a) {
-  IcpSE3 r;
-  r.q.w = a.q.w;
-  r.q.x = -a.q.x;
-  r.q.y = -a.q.y;
-  r.q.z = -a.q.z;
-  const F3 v = icp_qrot(r.q, a.t);
-  r.t = f3(-v.x, -v.y, -v.z);
-  return r;
-}
-// Eigen: quaternion <- rotation matrix
-__device__ inline IcpQuat icp_quat_from_matrix(const float m[3][3]) {
-  IcpQuat q;
-  float t = m[0][0] + m[1][1] + m[2][2];
-  if (t > 0.0f) {
-    t = sqrtf(t + 1.0f);
-    q.w = 0.5f * t;
-    t = 0.5f / t;
-    q.x = (m[2][1] - m[1][2]) * t;
-    q.y = (m[0][2] - m[2][0]) * t;
-    q.z = (m[1][0] - m[0][1]) * t;
-  } else {
-    int i = 0;
-    if (m[1][1] > m[0][0]) i = 1;
-    if (m[2][2] > m[i][i]) i = 2;
-    const int j = (i + 1) % 3, k = (j + 1) % 3;
-    float v[3];
-    t = sqrtf(m[i][i] - m[j][j] - m[k][k] + 1.0f);
-    v[i] = 0.5f * t;
-    t = 0.5f / t;
-    q.w = (m[k][j] - m[j][k]) * t;
-    v[j] = (m[j][i] + m[i][j]) * t;
-    v[k] = (m[k][i] + m[i][k]) * t;
-    q.x = v[0];
-    q.y = v[1];
-    q.z = v[2];
-  }
-  return q;
-}
-// minkindr RotationQuaternion::log / exp
-__device__ inline F3 icp_quat_log(const IcpQuat& q, float eps4_f) {
-  const F3 a = f3(q.x, q.y, q.z);
-  const float na = norm3(a), eta = q.w;
-  float scale;
-  if (fabsf(eta) < na) {
-    scale = eta >= 0.0f ? acosf(eta) / na : -acosf(-eta) / na;
-  } else {
-    const float s = fabsf(na) < eps4_f ? 1.0f + na * na * (float)(1.0 / 6.0) : asinf(na) / na;
-    scale = eta > 0.0f ? s : -s;
-  }
-  return scale3(a, 2.0f * scale);
-}
-__device__ inline IcpQuat icp_quat_exp(F3 d, double eps4_d) {
-  const double x = d.x, y = d.y, z = d.z;
-  const double theta = sqrt(x * x + y * y + z * z);
-  const double na = theta < eps4_d ? 0.5 + (theta * theta) * (1.0 / 48.0) : sin(theta * 0.5) / theta;
-  IcpQuat q;
-  q.w = (float)cos(theta * 0.5);
-  q.x = (float)(x * na);
-  q.y = (float)(y * na);
-  q.z = (float)(z * na);
-  return q;
-}
-
-// proper rotation maximising trace(R H) = V diag(1, 1, det) U^T of H = U S V^T (icp.h:160-177)
-__device__ inline void icp_rotation_from_h3(const float hf[3][3], float r[3][3]) {
-  double a[3][3], b[3][3], v[3][3];
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) a[i][j] = hf[i][j];
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) {
-      double s = 0;
-      for (int k = 0; k < 3; ++k) s += a[k][i] * a[k][j];
-      b[i][j] = s;
-      v[i][j] = i == j ? 1.0 : 0.0;
-    }
-  for (int sweep = 0; sweep < 60; ++sweep) {
-    double off = 0, diag = 0;
-    for (int i = 0; i < 3; ++i)
-      for (int j = 0; j < 3; ++j) {
-        if (i == j) {
-          diag += b[i][j] * b[i][j];
-        } else {
-          off += b[i][j] * b[i][j];
-        }
-      }
-    if (!(off > 1e-60) || off <= 1e-32 * diag) break;
-    for (int p = 0; p < 2; ++p)
-      for (int q = p + 1; q < 3; ++q) {
-        if (b[p][q] == 0.0) continue;
-        const double theta = (b[q][q] - b[p][p]) / (2.0 * b[p][q]);
-        const double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-        const double c = 1.0 / sqrt(t * t + 1.0), sn = t * c;
-        for (int k = 0; k < 3; ++k) {
-          const double bkp = b[k][p], bkq = b[k][q];
-          b[k][p] = c * bkp - sn * bkq;
-          b[k][q] = sn * bkp + c * bkq;
-        }
-        for (int k = 0; k < 3; ++k) {
-          const double bpk = b[p][k], bqk = b[q][k];
-          b[p][k] = c * bpk - sn * bqk;
-          b[q][k] = sn * bpk + c * bqk;
-        }
-        for (int k = 0; k < 3; ++k) {
-          const double vkp = v[k][p], vkq = v[k][q];
-          v[k][p] = c * vkp - sn * vkq;
-          v[k][q] = sn * vkp + c * vkq;
-        }
-      }
-  }
-  int order[3] = {0, 1, 2};
-  for (int i = 0; i < 3; ++i)
-    for (int j = i + 1; j < 3; ++j)
-      if (b[order[j]][order[j]] > b[order[i]][order[i]]) {
-        const int tmp = order[i];
-        order[i] = order[j];
-        order[j] = tmp;
-      }
-  double u[3][3], vs[3][3], sv[3];
-  for (int c = 0; c < 3; ++c) {
-    const double l = b[order[c]][order[c]];
-    sv[c] = sqrt(l > 0 ? l : 0.0);
-    for (int k = 0; k < 3; ++k) vs[k][c] = v[k][order[c]];
-  }
-  int good = 0;
-  for (int c = 0; c < 3; ++c) {
-    if (sv[c] > 1e-12 * (sv[0] > 0 ? sv[0] : 1.0) && sv[c] > 0) {
-      for (int i = 0; i < 3; ++i) {
-        double s = 0;
-        for (int k = 0; k < 3; ++k) s += a[i][k] * vs[k][c];
-        u[i][c] = s / sv[c];
-      }
-      good = c + 1;
-    } else {
-      break;
-    }
-  }
-  for (int c = good; c < 3; ++c)
-    for (int e = 0; e < 3; ++e) {
-      double w[3] = {e == 0 ? 1.0 : 0.0, e == 1 ? 1.0 : 0.0, e == 2 ? 1.0 : 0.0};
-      for (int p = 0; p < c; ++p) {
-        double dp = 0;
-        for (int i = 0; i < 3; ++i) dp += w[i] * u[i][p];
-        for (int i = 0; i < 3; ++i) w[i] -= dp * u[i][p];
-      }
-      const double nn = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
-      if (nn > 0.1) {
-        for (int i = 0; i < 3; ++i) u[i][c] = w[i] / sqrt(nn);
-        break;
-      }
-    }
-  float uf[3][3], vf[3][3];
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) {
-      uf[i][j] = (float)u[i][j];
-      vf[i][j] = (float)vs[i][j];
-    }
-  const float du = uf[0][0] * (uf[1][1] * uf[2][2] - uf[1][2] * uf[2][1]) - uf[0][1] * (uf[1][0] * uf[2][2] - uf[1][2] * uf[2][0]) +
-                   uf[0][2] * (uf[1][0] * uf[2][1] - uf[1][1] * uf[2][0]);
-  const float dv = vf[0][0] * (vf[1][1] * vf[2][2] - vf[1][2] * vf[2][1]) - vf[0][1] * (vf[1][0] * vf[2][2] - vf[1][2] * vf[2][0]) +
-                   vf[0][2] * (vf[1][0] * vf[2][1] - vf[1][1] * vf[2][0]);
-  if (du * dv < 0.0f)
-    for (int i = 0; i < 3; ++i) vf[i][2] = vf[i][2] * -1.0f;
-  for (int i = 0; i < 3; ++i)
-    for (int j = 0; j < 3; ++j) r[i][j] = vf[i][0] * uf[j][0] + vf[i][1] * uf[j][1] + vf[i][2] * uf[j][2];
-}
 
 // Interpolator::getNearestDistance (interpolator_inl.h:330-345) on the device map: the block by
 // Layer::computeBlockIndexFromCoordinates (core/layer.h:128-131), the voxel by
@@ -399,22 +205,8 @@ __global__ void __launch_bounds__(1024) k_icp(Tables tab, IcpParams P, const flo
         float* o = res + warp * 14;
         float ok = 0.0f;
         if (enough) {
-          float r[3][3] = {{1, 0, 0}, {0, 1, 0}, {0, 0, 1}};
-          if (!P.refine_roll_pitch) {
-            const float a = fadd(h[0][0], h[1][1]), b = fsub(h[0][1], h[1][0]);
-            const float nrm = fsqrt(fadd(fmul(a, a), fmul(b, b)));
-            const float c = fdiv(a, nrm), s = fdiv(b, nrm);
-            r[0][0] = c;
-            r[0][1] = -s;
-            r[1][0] = s;
-            r[1][1] = c;
-          } else {
-            icp_rotation_from_h3(h, r);
-          }
-          float sum = 0.0f;
-          for (int i = 0; i < 3; ++i)
-            for (int j = 0; j < 3; ++j) sum += r[i][j];
-          if (isfinite(sum)) {  // icp.h:183-186
+          float r[3][3];
+          if (icp_rotation(h, P.refine_roll_pitch != 0, r)) {
             const IcpQuat dq = icp_quat_from_matrix(r);
             const F3 dt = sub3(f3(tc[0], tc[1], tc[2]), icp_qrot(dq, f3(sc[0], sc[1], sc[2])));  // icp.cc:74-77
             o[1] = dq.w;
@@ -451,19 +243,7 @@ __global__ void __launch_bounds__(1024) k_icp(Tables tab, IcpParams P, const flo
         delta.q.y = o[3];
         delta.q.z = o[4];
         delta.t = f3(o[5], o[6], o[7]);
-        const IcpSE3 t_temp = icp_mul(delta, cur);
-        IcpSE3 d = icp_mul(icp_inv(cur), t_temp);
-        const F3 w3 = icp_quat_log(d.q, P.eps4_f);
-        const float lg[6] = {d.t.x, d.t.y, d.t.z, w3.x, w3.y, w3.z};
-        float wl[6];
-        for (int i = 0; i < 6; ++i) {
-          const float weight = fdiv(o[8 + i], fadd(s_base[i], o[8 + i]));
-          wl[i] = fmul(weight, lg[i]);
-          s_base[i] = fadd(s_base[i], o[8 + i]);
-        }
-        d.q = icp_quat_exp(f3(wl[3], wl[4], wl[5]), P.eps4_d);
-        d.t = f3(wl[0], wl[1], wl[2]);
-        cur = icp_mul(cur, d);
+        icp_fuse(cur, s_base, delta, o + 8, P.eps4_f, P.eps4_d);
         float* sp = snap + w * 7;
         sp[0] = cur.q.w;
         sp[1] = cur.q.x;
@@ -489,6 +269,69 @@ __global__ void __launch_bounds__(1024) k_icp(Tables tab, IcpParams P, const flo
     out[7] = 0.0f;
     *reinterpret_cast<unsigned long long*>(out + 8) = s_updates;
   }
+}
+
+// vbx_debug_icp_solve: one thread per item runs the per-batch arithmetic of k_icp on caller-given inputs
+__global__ void k_icp_debug_solve(uint32_t n, int refine_roll_pitch, float eps4_f, double eps4_d, const float* __restrict__ h,
+                                  const float* __restrict__ m, const float* __restrict__ q, const float* __restrict__ w,
+                                  float* __restrict__ r_out, int32_t* __restrict__ valid_out, float* __restrict__ q_out,
+                                  float* __restrict__ log_out, float* __restrict__ exp_out) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float hh[3][3], mm[3][3], r[3][3];
+  for (int k = 0; k < 9; ++k) {
+    hh[k / 3][k % 3] = h[9 * (size_t)i + k];
+    mm[k / 3][k % 3] = m[9 * (size_t)i + k];
+  }
+  valid_out[i] = icp_rotation(hh, refine_roll_pitch != 0, r) ? 1 : 0;
+  for (int k = 0; k < 9; ++k) r_out[9 * (size_t)i + k] = r[k / 3][k % 3];
+  const IcpQuat qm = icp_quat_from_matrix(mm);
+  IcpQuat qi;
+  qi.w = q[4 * (size_t)i];
+  qi.x = q[4 * (size_t)i + 1];
+  qi.y = q[4 * (size_t)i + 2];
+  qi.z = q[4 * (size_t)i + 3];
+  const F3 lg = icp_quat_log(qi, eps4_f);
+  const IcpQuat ex = icp_quat_exp(f3(w[3 * (size_t)i], w[3 * (size_t)i + 1], w[3 * (size_t)i + 2]), eps4_d);
+  const float qv[4] = {qm.w, qm.x, qm.y, qm.z}, lv[3] = {lg.x, lg.y, lg.z}, ev[4] = {ex.w, ex.x, ex.y, ex.z};
+  for (int k = 0; k < 4; ++k) q_out[4 * (size_t)i + k] = qv[k];
+  for (int k = 0; k < 3; ++k) log_out[3 * (size_t)i + k] = lv[k];
+  for (int k = 0; k < 4; ++k) exp_out[4 * (size_t)i + k] = ev[k];
+}
+
+int icp_debug_solve(vbx_ctx* c, uint32_t n, int refine_roll_pitch, const float* h, const float* m, const float* q,
+                    const float* w, float* r_out, int32_t* valid_out, float* q_out, float* log_out, float* exp_out) {
+  if (!n) return VBX_OK;
+  // one device allocation: h (9), m (9), q (4), w (3) in; r (9), q (4), log (3), exp (4) and valid out, per item
+  const size_t nn = n;
+  float* d = nullptr;
+  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&d), 46 * nn * sizeof(float)));
+  float *dh = d, *dm = dh + 9 * nn, *dq = dm + 9 * nn, *dw = dq + 4 * nn;
+  float *dr = dw + 3 * nn, *dqo = dr + 9 * nn, *dl = dqo + 4 * nn, *de = dl + 3 * nn;
+  int32_t* dv = reinterpret_cast<int32_t*>(de + 4 * nn);
+  cudaStream_t s = c->stream;
+  const float* hin[4] = {h, m, q, w};
+  float* din[4] = {dh, dm, dq, dw};
+  const size_t width_in[4] = {9, 9, 4, 3};
+  cudaError_t e = cudaSuccess;
+  for (int k = 0; k < 4 && e == cudaSuccess; ++k)
+    e = cudaMemcpyAsync(din[k], hin[k], width_in[k] * nn * sizeof(float), cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) {
+    k_icp_debug_solve<<<(n + 127) / 128, 128, 0, s>>>(n, refine_roll_pitch, std::pow(std::numeric_limits<float>::epsilon(), 0.25f),
+                                                      std::pow(std::numeric_limits<double>::epsilon(), 0.25), dh, dm, dq, dw, dr, dv,
+                                                      dqo, dl, de);
+    ++c->launches;
+    e = cudaGetLastError();
+  }
+  float* hout[4] = {r_out, q_out, log_out, exp_out};
+  const float* dout[4] = {dr, dqo, dl, de};
+  const size_t width_out[4] = {9, 4, 3, 4};
+  for (int k = 0; k < 4 && e == cudaSuccess; ++k)
+    e = cudaMemcpyAsync(hout[k], dout[k], width_out[k] * nn * sizeof(float), cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(valid_out, dv, nn * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  cudaFree(d);
+  return e == cudaSuccess ? VBX_OK : cuda_fail(c, e, "icp_debug_solve");
 }
 
 void icp_destroy(vbx_ctx* c) {
