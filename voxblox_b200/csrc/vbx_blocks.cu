@@ -150,16 +150,13 @@ __global__ void k_scatter_blocks(int layer, int serialized, const uint32_t* __re
 
 static int ensure_staging(vbx_ctx* c, size_t bytes, size_t slots) {
   if (bytes <= c->mirror_cap_bytes && slots <= c->mirror_cap_slots) return VBX_OK;
-  if (c->mirror_dev) cudaFree(c->mirror_dev);
-  if (c->mirror_host) cudaFreeHost(c->mirror_host);
-  if (c->mirror_slots) cudaFree(c->mirror_slots);
-  c->mirror_dev = c->mirror_host = nullptr;
-  c->mirror_slots = nullptr;
+  Holdings& h = c->own_staging;
+  h.release();
   c->mirror_cap_bytes = c->mirror_cap_slots = 0;
   const size_t want_b = std::max<size_t>(2 * bytes, 16u << 20), want_s = std::max<size_t>(2 * slots, 1024);
-  VBX_CUDA(c, cudaMalloc(&c->mirror_dev, want_b));
-  VBX_CUDA(c, cudaMallocHost(&c->mirror_host, want_b));
-  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->mirror_slots), want_s * sizeof(uint32_t)));
+  VBX_CUDA(c, h.dev(&c->mirror_dev, want_b));
+  VBX_CUDA(c, h.host(&c->mirror_host, want_b));
+  VBX_CUDA(c, h.dev(&c->mirror_slots, want_s));
   c->mirror_cap_bytes = want_b;
   c->mirror_cap_slots = want_s;
   return VBX_OK;
@@ -614,11 +611,10 @@ int gather_updated_device(vbx_ctx* c, int layer, int updated_mask, int clear_mas
   if (items.empty() || items.size() > cap) return VBX_OK;  // (too small a buffer: nothing copied or cleared)
   const size_t m = items.size();
   if (m > c->xfer_cap_slots) {
-    if (c->xfer_slots) cudaFree(c->xfer_slots);
-    c->xfer_slots = nullptr;
+    c->own_xfer.release();
     c->xfer_cap_slots = 0;
     const size_t want = std::max<size_t>(2 * m, 1024);
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->xfer_slots), want * sizeof(uint32_t)));
+    VBX_CUDA(c, c->own_xfer.dev(&c->xfer_slots, want));
     c->xfer_cap_slots = want;
   }
   std::vector<int32_t> idx(3 * m);

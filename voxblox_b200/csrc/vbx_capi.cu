@@ -132,85 +132,58 @@ int drain_async(vbx_ctx* c) {
   return VBX_OK;
 }
 
-template <typename T>
-static cudaError_t dmalloc(T** p, size_t count) {
-  return cudaMalloc(reinterpret_cast<void**>(p), count * sizeof(T));
-}
-
 // Everything a hand-off set owns except the pipeline's streams and events (ensure_async).  Its private block
 // table is zeroed here, once; afterwards every call clears the positions it used.
-static int alloc_set(vbx_ctx* c, vbx_ctx::ScratchSet& S) {
+static int alloc_set(vbx_ctx* c, Holdings& h, vbx_ctx::ScratchSet& S) {
   const size_t np = c->max_points, nu = c->max_updates;
-  VBX_CUDA(c, dmalloc(&S.ray_p, np));
-  VBX_CUDA(c, dmalloc(&S.ray_a, np));
-  VBX_CUDA(c, dmalloc(&S.ray_c, np));
-  VBX_CUDA(c, dmalloc(&S.ray_list, np));
-  VBX_CUDA(c, dmalloc(&S.head_list, np));
-  VBX_CUDA(c, dmalloc(&S.touched_list, c->tab.touched_cap));
-  VBX_CUDA(c, dmalloc(&S.cnt, np + 1));
-  VBX_CUDA(c, dmalloc(&S.off, np + 1));
-  VBX_CUDA(c, dmalloc(&S.d_state, 1));
-  VBX_CUDA(c, cudaMallocHost(reinterpret_cast<void**>(&S.h_state), sizeof(ScanState)));
-  if (int rc = alloc_scan_args(c, S)) return rc;
-  VBX_CUDA(c, dmalloc(&S.d_xyz, 3 * np));
-  VBX_CUDA(c, dmalloc(&S.d_rgba, 4 * np));
-  VBX_CUDA(c, dmalloc(&S.pkeys0, np));
+  VBX_CUDA(c, h.dev(&S.ray_p, np));
+  VBX_CUDA(c, h.dev(&S.ray_a, np));
+  VBX_CUDA(c, h.dev(&S.ray_c, np));
+  VBX_CUDA(c, h.dev(&S.ray_list, np));
+  VBX_CUDA(c, h.dev(&S.head_list, np));
+  VBX_CUDA(c, h.dev(&S.touched_list, c->tab.touched_cap));
+  VBX_CUDA(c, h.dev(&S.cnt, np + 1));
+  VBX_CUDA(c, h.dev(&S.off, np + 1));
+  VBX_CUDA(c, h.dev(&S.d_state, 1));
+  VBX_CUDA(c, h.host(&S.h_state, 1));
+  if (int rc = alloc_scan_args(c, h, S)) return rc;
+  VBX_CUDA(c, h.dev(&S.d_xyz, 3 * np));
+  VBX_CUDA(c, h.dev(&S.d_rgba, 4 * np));
+  VBX_CUDA(c, h.dev(&S.pkeys0, np));
   for (int i = 0; i < 2; ++i) {
-    VBX_CUDA(c, dmalloc(&S.ckeys[i], nu));
-    VBX_CUDA(c, dmalloc(&S.cvals[i], nu));
+    VBX_CUDA(c, h.dev(&S.ckeys[i], nu));
+    VBX_CUDA(c, h.dev(&S.cvals[i], nu));
   }
-  VBX_CUDA(c, dmalloc(&S.long_list, nu / 32 + 1));
-  VBX_CUDA(c, dmalloc(&S.long_end, nu / 32 + 1));
-  VBX_CUDA(c, dmalloc(&S.keep_bits, nu / 32 + 1));
-  VBX_CUDA(c, dmalloc(&S.sort_plan1, 1));
-  VBX_CUDA(c, dmalloc(&S.sort_status1, (size_t)4 * c->sort_tiles_cap[1] * kRadix));
+  VBX_CUDA(c, h.dev(&S.long_list, nu / 32 + 1));
+  VBX_CUDA(c, h.dev(&S.long_end, nu / 32 + 1));
+  VBX_CUDA(c, h.dev(&S.keep_bits, nu / 32 + 1));
+  VBX_CUDA(c, h.dev(&S.sort_plan1, 1));
+  VBX_CUDA(c, h.dev(&S.sort_status1, (size_t)4 * c->sort_tiles_cap[1] * kRadix));
   ScanBlocks& b = S.blocks;
   b.cap = c->tab.touched_cap;
   uint32_t size = 1;
   while (size < 2 * b.cap) size <<= 1;
   b.mask = size - 1;
-  VBX_CUDA(c, dmalloc(&b.table, size));
-  VBX_CUDA(c, dmalloc(&b.keys, b.cap));
-  VBX_CUDA(c, dmalloc(&b.pos, b.cap));
+  VBX_CUDA(c, h.dev(&b.table, size));
+  VBX_CUDA(c, h.dev(&b.keys, b.cap));
+  VBX_CUDA(c, h.dev(&b.pos, b.cap));
   VBX_CUDA(c, cudaMemsetAsync(b.table, 0, (size_t)size * sizeof(uint32_t), c->stream));
   VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), c->stream));
   VBX_CUDA(c, cudaStreamSynchronize(c->stream));
   return VBX_OK;
 }
 
-static void free_set(vbx_ctx::ScratchSet& S) {
-  const ScanBlocks& b = S.blocks;
-  void* dev[] = {S.ray_p, S.ray_a, S.ray_c, S.ray_list, S.head_list, S.touched_list, b.table, b.keys, b.pos, S.cnt,
-                 S.off, S.d_state, S.d_args, S.d_xyz, S.d_rgba, S.pkeys0, S.ckeys[0], S.ckeys[1], S.cvals[0],
-                 S.cvals[1], S.long_list, S.long_end, S.keep_bits, S.sort_plan1, S.sort_status1};
-  for (void* p : dev) {
-    if (p) cudaFree(p);
-  }
-  if (S.h_state) cudaFreeHost(S.h_state);
-  if (S.h_args) cudaFreeHost(S.h_args);
-  for (auto& per_lane : S.graph) {
-    for (vbx_ctx::ScanGraph& G : per_lane) {
-      if (G.exec) cudaGraphExecDestroy(G.exec);
-      if (G.graph) cudaGraphDestroy(G.graph);
-    }
-  }
-  if (S.stream) cudaStreamDestroy(S.stream);
-  for (cudaEvent_t e : {S.copy_done, S.walked, S.sorted, S.applied, S.back_done, S.front_start, S.front_done}) {
-    if (e) cudaEventDestroy(e);
-  }
-}
-
 // Everything a front lane owns except the pipeline's stream and event (ensure_async).
-static int alloc_lane(vbx_ctx* c, vbx_ctx::FrontLane& F) {
+static int alloc_lane(vbx_ctx* c, Holdings& h, vbx_ctx::FrontLane& F) {
   const size_t np = c->max_points;
-  VBX_CUDA(c, dmalloc(&F.pkeys1, np));
-  VBX_CUDA(c, dmalloc(&F.pvals[0], np));
-  VBX_CUDA(c, dmalloc(&F.pvals[1], np));
-  VBX_CUDA(c, dmalloc(&F.sort_plan0, 1));
-  VBX_CUDA(c, dmalloc(&F.sort_status0, (size_t)8 * c->sort_tiles_cap[0] * kRadix));
-  VBX_CUDA(c, dmalloc(&F.scan_status, (np + 1) / kScanTile + 4));
-  VBX_CUDA(c, dmalloc(&F.big_list, np / 256 + 2));
-  VBX_CUDA(c, dmalloc(&F.first_bits, 2 * (np / 32 + 2)));
+  VBX_CUDA(c, h.dev(&F.pkeys1, np));
+  VBX_CUDA(c, h.dev(&F.pvals[0], np));
+  VBX_CUDA(c, h.dev(&F.pvals[1], np));
+  VBX_CUDA(c, h.dev(&F.sort_plan0, 1));
+  VBX_CUDA(c, h.dev(&F.sort_status0, (size_t)8 * c->sort_tiles_cap[0] * kRadix));
+  VBX_CUDA(c, h.dev(&F.scan_status, (np + 1) / kScanTile + 4));
+  VBX_CUDA(c, h.dev(&F.big_list, np / 256 + 2));
+  VBX_CUDA(c, h.dev(&F.first_bits, 2 * (np / 32 + 2)));
   VBX_CUDA(c, cudaMemsetAsync(F.first_bits, 0, 2 * (np / 32 + 2) * sizeof(uint32_t), c->stream));
   // k_bundle_order's tables (vbx_order.cuh), for the bucket count after np insertions
   OrderScratch& g = F.order_scratch;
@@ -218,37 +191,20 @@ static int alloc_lane(vbx_ctx* c, vbx_ctx::FrontLane& F) {
   uint32_t buckets = 1;
   for (int k = 0; k < c->rehash.count && c->rehash.m[k] < np; ++k) buckets = c->rehash.n[k];
   g.bucket_cap = buckets;
-  VBX_CUDA(c, dmalloc(&g.h, 2 * np));
-  VBX_CUDA(c, dmalloc(&g.tau, np));
-  VBX_CUDA(c, dmalloc(&g.tau2, np));
-  VBX_CUDA(c, dmalloc(&g.next, np));
-  VBX_CUDA(c, dmalloc(&g.bkt, np));
-  VBX_CUDA(c, dmalloc(&g.A, np));
-  VBX_CUDA(c, dmalloc(&g.bhead, (size_t)buckets));
-  VBX_CUDA(c, dmalloc(&g.head_of, 2 * np));
-  VBX_CUDA(c, dmalloc(&g.wp, 2 * (np / 32 + 2)));
-  VBX_CUDA(c, dmalloc(&g.cta_tot, 64));
-  VBX_CUDA(c, cudaStreamCreateWithPriority(&F.side, cudaStreamNonBlocking, c->prio_lo));
-  VBX_CUDA(c, cudaEventCreateWithFlags(&F.ev_fork, cudaEventDisableTiming));
-  VBX_CUDA(c, cudaEventCreateWithFlags(&F.ev_join, cudaEventDisableTiming));
+  VBX_CUDA(c, h.dev(&g.h, 2 * np));
+  VBX_CUDA(c, h.dev(&g.tau, np));
+  VBX_CUDA(c, h.dev(&g.tau2, np));
+  VBX_CUDA(c, h.dev(&g.next, np));
+  VBX_CUDA(c, h.dev(&g.bkt, np));
+  VBX_CUDA(c, h.dev(&g.A, np));
+  VBX_CUDA(c, h.dev(&g.bhead, (size_t)buckets));
+  VBX_CUDA(c, h.dev(&g.head_of, 2 * np));
+  VBX_CUDA(c, h.dev(&g.wp, 2 * (np / 32 + 2)));
+  VBX_CUDA(c, h.dev(&g.cta_tot, 64));
+  VBX_CUDA(c, h.stream(&F.side, cudaStreamNonBlocking, c->prio_lo));
+  VBX_CUDA(c, h.event(&F.ev_fork, cudaEventDisableTiming));
+  VBX_CUDA(c, h.event(&F.ev_join, cudaEventDisableTiming));
   return VBX_OK;
-}
-
-static void free_lane(vbx_ctx::FrontLane& F) {
-  const OrderScratch& g = F.order_scratch;
-  void* dev[] = {F.pkeys1, F.pvals[0], F.pvals[1], F.sort_plan0, F.sort_status0, F.scan_status, F.big_list, F.first_bits,
-                 g.h, g.tau, g.tau2, g.next, g.bkt, g.A, g.bhead, g.head_of, g.wp, g.cta_tot};
-  for (void* p : dev) {
-    if (p) cudaFree(p);
-  }
-  if (F.side) {
-    cudaStreamSynchronize(F.side);
-    cudaStreamDestroy(F.side);
-  }
-  for (cudaEvent_t e : {F.ev_fork, F.ev_join, F.done}) {
-    if (e) cudaEventDestroy(e);
-  }
-  if (F.stream) cudaStreamDestroy(F.stream);
 }
 
 }  // namespace vbx
@@ -318,12 +274,8 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
     return VBX_E_INVALID;
   }
   *out = c;  // from here on the caller can read vbx_last_error and must vbx_destroy
-#define CK(expr)                                   \
-  do {                                             \
-    cudaError_t _e = (expr);                       \
-    if (_e != cudaSuccess) return cuda_fail(c, _e, #expr); \
-  } while (0)
-  CK(cudaSetDevice(c->device));
+  Holdings& h = c->own_core;
+  VBX_CUDA(c, cudaSetDevice(c->device));
   {
     int sms = 0;
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device) == cudaSuccess && sms > 0) c->grid_sms = (unsigned int)sms;
@@ -332,17 +284,17 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
   // stream priorities for the pipelined path: the stages that run in submission order (apply, then
   // the ray walk) are the pipeline's bottleneck, so their thread blocks go first
   int prio_lo = 0, prio_hi = 0;
-  CK(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));  // numerically lower = higher priority
+  VBX_CUDA(c, cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));  // numerically lower = higher priority
   c->prio_lo = prio_lo;
   c->prio_hi = prio_hi;
-  CK(cudaStreamCreateWithPriority(&c->stream, cudaStreamNonBlocking, prio_hi));
-  CK(cudaStreamCreateWithFlags(&c->stream_c, cudaStreamNonBlocking));
-  CK(cudaStreamCreateWithFlags(&c->stream_c2, cudaStreamNonBlocking));
-  CK(cudaEventCreate(&c->ev0));
-  CK(cudaEventCreate(&c->ev1));
-  CK(cudaEventCreate(&c->tev0));
-  CK(cudaEventCreate(&c->tev1));
-  for (int i = 0; i < 20; ++i) CK(cudaEventCreate(&c->sev[i]));
+  VBX_CUDA(c, h.stream(&c->stream, cudaStreamNonBlocking, prio_hi));
+  VBX_CUDA(c, h.stream(&c->stream_c, cudaStreamNonBlocking));
+  VBX_CUDA(c, h.stream(&c->stream_c2, cudaStreamNonBlocking));
+  VBX_CUDA(c, h.event(&c->ev0));
+  VBX_CUDA(c, h.event(&c->ev1));
+  VBX_CUDA(c, h.event(&c->tev0));
+  VBX_CUDA(c, h.event(&c->tev1));
+  for (int i = 0; i < 20; ++i) VBX_CUDA(c, h.event(&c->sev[i]));
   uint32_t hcap = 1;
   while (hcap < 2 * o.max_blocks) hcap <<= 1;
   c->hcap = hcap;
@@ -350,43 +302,42 @@ int vbx_create(const vbx_tsdf_config* cfg, float voxel_size, int voxels_per_side
   std::memset(&t, 0, sizeof(t));
   t.hmask = hcap - 1;
   t.max_blocks = o.max_blocks;
-  CK(dmalloc(&t.hkeys, hcap));
-  CK(dmalloc(&t.hslot, hcap));
-  CK(dmalloc(&t.new_list, o.max_blocks));
+  VBX_CUDA(c, h.dev(&t.hkeys, hcap));
+  VBX_CUDA(c, h.dev(&t.hslot, hcap));
+  VBX_CUDA(c, h.dev(&t.new_list, o.max_blocks));
   // one local id per block a call touches (vbx_hash.cuh, scan_block_id), with headroom past the pool;
   // (id, voxel) must fit a 32-bit record key
   t.touched_cap = (uint32_t)std::min<uint64_t>((uint64_t)o.max_blocks + 65536u, (0xffffffffull >> (3 * c->L)) - 1);
   t.vox_per_block = c->vox_per_block;
-  CK(dmalloc(&t.slot_key, o.max_blocks));
-  CK(dmalloc(&t.slot_updated, o.max_blocks));
-  CK(dmalloc(&t.slot_esdf_updated, o.max_blocks));
-  CK(dmalloc(&t.slot_has_esdf, o.max_blocks));
-  CK(dmalloc(&t.tsdf, (size_t)o.max_blocks * c->vox_per_block));
-  CK(cudaMemsetAsync(t.hkeys, 0xff, (size_t)hcap * sizeof(uint64_t), c->stream));
-  CK(cudaMemsetAsync(t.hslot, 0xff, (size_t)hcap * sizeof(int32_t), c->stream));
-  CK(cudaMemsetAsync(t.slot_updated, 0, o.max_blocks, c->stream));
-  CK(cudaMemsetAsync(t.slot_esdf_updated, 0, o.max_blocks, c->stream));
-  CK(cudaMemsetAsync(t.slot_has_esdf, 0, o.max_blocks, c->stream));
+  VBX_CUDA(c, h.dev(&t.slot_key, o.max_blocks));
+  VBX_CUDA(c, h.dev(&t.slot_updated, o.max_blocks));
+  VBX_CUDA(c, h.dev(&t.slot_esdf_updated, o.max_blocks));
+  VBX_CUDA(c, h.dev(&t.slot_has_esdf, o.max_blocks));
+  VBX_CUDA(c, h.dev(&t.tsdf, (size_t)o.max_blocks * c->vox_per_block));
+  VBX_CUDA(c, cudaMemsetAsync(t.hkeys, 0xff, (size_t)hcap * sizeof(uint64_t), c->stream));
+  VBX_CUDA(c, cudaMemsetAsync(t.hslot, 0xff, (size_t)hcap * sizeof(int32_t), c->stream));
+  VBX_CUDA(c, cudaMemsetAsync(t.slot_updated, 0, o.max_blocks, c->stream));
+  VBX_CUDA(c, cudaMemsetAsync(t.slot_esdf_updated, 0, o.max_blocks, c->stream));
+  VBX_CUDA(c, cudaMemsetAsync(t.slot_has_esdf, 0, o.max_blocks, c->stream));
   // new Block: voxels default-constructed = all zero bytes (core/voxel.h:12-16)
-  CK(cudaMemsetAsync(t.tsdf, 0, (size_t)o.max_blocks * c->vox_per_block * sizeof(TsdfVoxel), c->stream));
+  VBX_CUDA(c, cudaMemsetAsync(t.tsdf, 0, (size_t)o.max_blocks * c->vox_per_block * sizeof(TsdfVoxel), c->stream));
   const size_t np = c->max_points;
-  CK(dmalloc(&c->order, np));
-  CK(dmalloc(&c->order_inv, np));
+  VBX_CUDA(c, h.dev(&c->order, np));
+  VBX_CUDA(c, h.dev(&c->order_inv, np));
   if (int rc = init_bundle_order(c)) return rc;
   c->sort_tiles_cap[0] = (uint32_t)((np + kSortTile - 1) / kSortTile);
   c->sort_tiles_cap[1] = (uint32_t)((c->max_updates + kSortTile - 1) / kSortTile);
-  CK(dmalloc(&c->set_start, kApproxSetWords));
-  CK(dmalloc(&c->set_observed, kApproxSetWords));
+  VBX_CUDA(c, h.dev(&c->set_start, kApproxSetWords));
+  VBX_CUDA(c, h.dev(&c->set_observed, kApproxSetWords));
   if (int rc = init_fast_sets(c, c->stream)) return rc;
-  CK(dmalloc(&c->d_nblocks, 2));
-  CK(cudaMemsetAsync(c->d_nblocks, 0, 2 * sizeof(uint32_t), c->stream));
-  CK(dmalloc(&c->d_hold, 1));
-  CK(cudaMemsetAsync(c->d_hold, 0, sizeof(uint32_t), c->stream));
+  VBX_CUDA(c, h.dev(&c->d_nblocks, 2));
+  VBX_CUDA(c, cudaMemsetAsync(c->d_nblocks, 0, 2 * sizeof(uint32_t), c->stream));
+  VBX_CUDA(c, h.dev(&c->d_hold, 1));
+  VBX_CUDA(c, cudaMemsetAsync(c->d_hold, 0, sizeof(uint32_t), c->stream));
   // the synchronous calls' scratch; ensure_async allocates the other sets and lanes
-  if (int rc = alloc_set(c, c->set[0])) return rc;
-  if (int rc = alloc_lane(c, c->lane[0])) return rc;
-  CK(cudaStreamSynchronize(c->stream));
-#undef CK
+  if (int rc = alloc_set(c, h, c->set[0])) return rc;
+  if (int rc = alloc_lane(c, h, c->lane[0])) return rc;
+  VBX_CUDA(c, cudaStreamSynchronize(c->stream));
   return VBX_OK;
 }
 
@@ -396,46 +347,42 @@ namespace vbx {
 // First asynchronous submission: the remaining hand-off sets, the second front lane, streams, events.
 int ensure_async(vbx_ctx* c) {
   if (c->async_ready) return VBX_OK;
-#define CK(expr)                                           \
-  do {                                                     \
-    cudaError_t _e = (expr);                               \
-    if (_e != cudaSuccess) return cuda_fail(c, _e, #expr); \
-  } while (0)
+  Holdings& h = c->own_async;
+  h.release();  // whatever a failed earlier call made
   if (const char* e = std::getenv("VBX_ASYNC_SETS")) c->sets_in_use = std::max(2, std::min(std::atoi(e), (int)vbx_ctx::kSets));
   if (const char* e = std::getenv("VBX_ASYNC_LANES")) c->lanes_in_use = std::max(1, std::min(std::atoi(e), (int)vbx_ctx::kLanes));
-  CK(cudaStreamCreateWithPriority(&c->stream_e, cudaStreamNonBlocking, std::min(c->prio_lo, c->prio_hi + 1)));
-  CK(cudaStreamCreateWithPriority(&c->stream_s, cudaStreamNonBlocking, std::min(c->prio_lo, c->prio_hi + 2)));
-  for (cudaEvent_t& e : c->cap_ev) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  VBX_CUDA(c, h.stream(&c->stream_e, cudaStreamNonBlocking, std::min(c->prio_lo, c->prio_hi + 1)));
+  VBX_CUDA(c, h.stream(&c->stream_s, cudaStreamNonBlocking, std::min(c->prio_lo, c->prio_hi + 2)));
+  for (cudaEvent_t& e : c->cap_ev) VBX_CUDA(c, h.event(&e, cudaEventDisableTiming));
   for (int l = 0; l < c->lanes_in_use; ++l) {
     vbx_ctx::FrontLane& F = c->lane[l];
-    CK(cudaStreamCreateWithPriority(&F.stream, cudaStreamNonBlocking, c->prio_lo));
-    CK(cudaEventCreateWithFlags(&F.done, cudaEventDisableTiming));
+    VBX_CUDA(c, h.stream(&F.stream, cudaStreamNonBlocking, c->prio_lo));
+    VBX_CUDA(c, h.event(&F.done, cudaEventDisableTiming));
     if (l == 0) continue;
-    if (int rc = alloc_lane(c, F)) return rc;
+    if (int rc = alloc_lane(c, h, F)) return rc;
   }
   // diagnostic: with VBX_ASYNC_TIMELINE set the hand-off events keep timestamps (vbx_debug_async_timeline)
   c->timeline = std::getenv("VBX_ASYNC_TIMELINE") != nullptr;
   const unsigned int evf = c->timeline ? cudaEventDefault : cudaEventDisableTiming;
   if (c->timeline) {
-    CK(cudaEventCreate(&c->timeline_ref));
-    CK(cudaEventRecord(c->timeline_ref, c->stream));
+    VBX_CUDA(c, h.event(&c->timeline_ref));
+    VBX_CUDA(c, cudaEventRecord(c->timeline_ref, c->stream));
   }
   for (int k = 0; k < c->sets_in_use; ++k) {
     vbx_ctx::ScratchSet& S = c->set[k];
-    CK(cudaStreamCreateWithFlags(&S.stream, cudaStreamNonBlocking));
-    CK(cudaEventCreateWithFlags(&S.copy_done, evf));
-    CK(cudaEventCreateWithFlags(&S.walked, evf));
-    CK(cudaEventCreateWithFlags(&S.sorted, evf));
-    CK(cudaEventCreateWithFlags(&S.back_done, evf));
-    CK(cudaEventCreateWithFlags(&S.applied, evf));
+    VBX_CUDA(c, h.stream(&S.stream, cudaStreamNonBlocking));
+    VBX_CUDA(c, h.event(&S.copy_done, evf));
+    VBX_CUDA(c, h.event(&S.walked, evf));
+    VBX_CUDA(c, h.event(&S.sorted, evf));
+    VBX_CUDA(c, h.event(&S.back_done, evf));
+    VBX_CUDA(c, h.event(&S.applied, evf));
     if (c->timeline) {
-      CK(cudaEventCreate(&S.front_start));
-      CK(cudaEventCreate(&S.front_done));
+      VBX_CUDA(c, h.event(&S.front_start));
+      VBX_CUDA(c, h.event(&S.front_done));
     }
     if (k == 0) continue;
-    if (int rc = alloc_set(c, S)) return rc;
+    if (int rc = alloc_set(c, h, S)) return rc;
   }
-#undef CK
   c->async_ready = true;
   return VBX_OK;
 }
@@ -446,47 +393,17 @@ extern "C" {
 void vbx_destroy(vbx_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
-  if (c->stream) cudaStreamSynchronize(c->stream);
-  if (c->stream_c) cudaStreamSynchronize(c->stream_c);
-  if (c->stream_c2) cudaStreamSynchronize(c->stream_c2);
-  for (int k = 0; k < vbx_ctx::kSets; ++k) {
-    if (c->set[k].stream) cudaStreamSynchronize(c->set[k].stream);
+  // every stream's work ends before the owners free what it reads (vbx_ctx::own_*)
+  for (cudaStream_t s : {c->stream, c->stream_c, c->stream_c2}) {
+    if (s) cudaStreamSynchronize(s);
   }
-  for (int l = 0; l < vbx_ctx::kLanes; ++l) {
-    if (c->lane[l].stream) cudaStreamSynchronize(c->lane[l].stream);
+  for (const vbx_ctx::ScratchSet& S : c->set) {
+    if (S.stream) cudaStreamSynchronize(S.stream);
   }
-  esdf_destroy(c);
-  mesh_destroy(c);
-  icp_destroy(c);
-  Tables& t = c->tab;
-  void* ptrs[] = {t.hkeys,    t.hslot,        t.new_list,   t.slot_key,     t.slot_updated,
-                  t.slot_esdf_updated, t.slot_has_esdf, t.tsdf, c->order, c->order_inv, c->set_start,
-                  c->set_observed, c->d_nblocks, c->d_hold};
-  for (void* p : ptrs) {
-    if (p) cudaFree(p);
+  for (const vbx_ctx::FrontLane& F : c->lane) {
+    if (F.stream) cudaStreamSynchronize(F.stream);
+    if (F.side) cudaStreamSynchronize(F.side);
   }
-  if (c->mirror_dev) cudaFree(c->mirror_dev);
-  if (c->mirror_host) cudaFreeHost(c->mirror_host);
-  if (c->mirror_slots) cudaFree(c->mirror_slots);
-  if (c->xfer_slots) cudaFree(c->xfer_slots);
-  for (vbx_ctx::ScratchSet& S : c->set) free_set(S);
-  for (vbx_ctx::FrontLane& F : c->lane) free_lane(F);
-  if (c->timeline_ref) cudaEventDestroy(c->timeline_ref);
-  if (c->ev0) cudaEventDestroy(c->ev0);
-  if (c->ev1) cudaEventDestroy(c->ev1);
-  if (c->tev0) cudaEventDestroy(c->tev0);
-  if (c->tev1) cudaEventDestroy(c->tev1);
-  for (int i = 0; i < 20; ++i) {
-    if (c->sev[i]) cudaEventDestroy(c->sev[i]);
-  }
-  if (c->stream) cudaStreamDestroy(c->stream);
-  if (c->stream_e) cudaStreamDestroy(c->stream_e);
-  if (c->stream_s) cudaStreamDestroy(c->stream_s);
-  for (cudaEvent_t e : c->cap_ev) {
-    if (e) cudaEventDestroy(e);
-  }
-  if (c->stream_c) cudaStreamDestroy(c->stream_c);
-  if (c->stream_c2) cudaStreamDestroy(c->stream_c2);
   delete c;
 }
 

@@ -6,6 +6,7 @@
 #include <stdint.h>
 
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <unordered_set>
 #include <vector>
@@ -190,6 +191,70 @@ __host__ __device__ inline uint32_t hash64(uint64_t k) {
   k ^= k >> 33;
   return (uint32_t)k;
 }
+
+// The owner of a group of CUDA resources that share one lifetime: the only code that allocates, creates, frees
+// or destroys them.  Each method stores the new handle in the field it is given and records that field's
+// address; release() frees everything recorded, newest first, nulls each field and forgets it.  The fields stay
+// plain pointers and handles (Tables, ScanBlocks and OrderScratch go to kernels by value), so a held field must
+// not move: the context's fields never do (vbx_ctx is allocated once).  Each method returns the CUDA error.
+class Holdings {
+ public:
+  Holdings() = default;
+  Holdings(const Holdings&) = delete;
+  Holdings& operator=(const Holdings&) = delete;
+  ~Holdings() { release(); }
+
+  template <typename T>
+  cudaError_t dev(T** p, size_t count) {  // device memory for count elements (bytes for void)
+    return keep(cudaMalloc(reinterpret_cast<void**>(p), count * sizeof(Unit<T>)), kDevice, p);
+  }
+  template <typename T>
+  cudaError_t host(T** p, size_t count) {  // page-locked host memory
+    return keep(cudaMallocHost(reinterpret_cast<void**>(p), count * sizeof(Unit<T>)), kHost, p);
+  }
+  cudaError_t stream(cudaStream_t* s, unsigned int flags) { return keep(cudaStreamCreateWithFlags(s, flags), kStream, s); }
+  cudaError_t stream(cudaStream_t* s, unsigned int flags, int priority) {
+    return keep(cudaStreamCreateWithPriority(s, flags, priority), kStream, s);
+  }
+  cudaError_t event(cudaEvent_t* e) { return keep(cudaEventCreate(e), kEvent, e); }
+  cudaError_t event(cudaEvent_t* e, unsigned int flags) { return keep(cudaEventCreateWithFlags(e, flags), kEvent, e); }
+  // an instantiated graph and its executable: the exec is destroyed first
+  void graph(cudaGraph_t* g, cudaGraphExec_t* x) {
+    held_.push_back({kGraph, g});
+    held_.push_back({kGraphExec, x});
+  }
+
+  void release() {
+    for (auto it = held_.rbegin(); it != held_.rend(); ++it) {
+      void** field = static_cast<void**>(it->field);
+      if (!*field) continue;
+      switch (it->kind) {
+        case kDevice: cudaFree(*field); break;
+        case kHost: cudaFreeHost(*field); break;
+        case kStream: cudaStreamDestroy(static_cast<cudaStream_t>(*field)); break;
+        case kEvent: cudaEventDestroy(static_cast<cudaEvent_t>(*field)); break;
+        case kGraph: cudaGraphDestroy(static_cast<cudaGraph_t>(*field)); break;
+        case kGraphExec: cudaGraphExecDestroy(static_cast<cudaGraphExec_t>(*field)); break;
+      }
+      *field = nullptr;
+    }
+    held_.clear();
+  }
+
+ private:
+  template <typename T>
+  using Unit = std::conditional_t<std::is_void_v<T>, char, T>;
+  enum Kind { kDevice, kHost, kStream, kEvent, kGraph, kGraphExec };
+  struct Held {
+    Kind kind;
+    void* field;  // T**, cudaStream_t*, ...: every handle is a pointer
+  };
+  cudaError_t keep(cudaError_t e, Kind kind, void* field) {
+    if (e == cudaSuccess) held_.push_back({kind, field});
+    return e;
+  }
+  std::vector<Held> held_;
+};
 
 }  // namespace vbx
 
@@ -386,6 +451,17 @@ struct vbx_ctx {
   double stage_ms[16] = {0};
   uint64_t stage_calls[16] = {0};
   std::string err;
+  // The owners of the fields above, one per lifetime.  Declared last, so that they are destroyed first,
+  // while every field they null is still alive; vbx_destroy synchronises the streams before.
+  vbx::Holdings own_core;          // vbx_create: the map, the Fast sets, set 0 / lane 0 buffers, main streams and events
+  vbx::Holdings own_async;         // ensure_async: every set's and lane's streams and events, the buffers of sets / lanes
+                                   // 1 and up, stream_e / stream_s / cap_ev, the timeline events; the captured scan graphs
+  vbx::Holdings own_esdf;          // esdf_create, and esdf_fe
+  vbx::Holdings own_mesh_blocks;   // mesh_generate's per-block buffers
+  vbx::Holdings own_mesh_vertices;  // ... and its vertex buffers
+  vbx::Holdings own_icp;           // icp_run's buffers
+  vbx::Holdings own_staging;       // mirror_dev / mirror_host / mirror_slots
+  vbx::Holdings own_xfer;          // xfer_slots
 };
 
 namespace vbx {
@@ -421,9 +497,6 @@ int gather_updated_device(vbx_ctx* c, int layer, int updated_mask, int clear_mas
                           void* d_voxels, uint64_t cap, uint64_t* n);
 int upload_blocks_device(vbx_ctx* c, int layer, const int32_t* d_idx3, uint64_t m, const void* d_voxels,
                          uint8_t updated_bits);
-int esdf_destroy(vbx_ctx* c);
-void mesh_destroy(vbx_ctx* c);
-void icp_destroy(vbx_ctx* c);
 int icp_debug_solve(vbx_ctx* c, uint32_t n, int refine_roll_pitch, const float* h, const float* m, const float* q,
                     const float* w, float* r_out, int32_t* valid_out, float* q_out, float* log_out, float* exp_out);
 int icp_run(vbx_ctx* c, const vbx_icp_config* cfg, const float* points, int on_device, uint64_t n, const float q[4],
@@ -439,7 +512,8 @@ int set_n_blocks(vbx_ctx* c, uint32_t n);
 int init_bundle_order(vbx_ctx* c);     // rehash schedule + shared-memory opt-in of k_bundle_order
 int rebuild_hash(vbx_ctx* c);          // block hash rebuilt from slot_key (after removals / a pool overflow)
 void harvest_async(vbx_ctx* c, vbx_ctx::ScratchSet& S);  // collect a finished asynchronous scan's results
-int alloc_scan_args(vbx_ctx* c, vbx_ctx::ScratchSet& S);  // the set's argument block, device + page-locked host
+// the set's argument block, device + page-locked host, held by h
+int alloc_scan_args(vbx_ctx* c, Holdings& h, vbx_ctx::ScratchSet& S);
 
 // Where a scan's work is enqueued (vbx_tsdf.cu): its hand-off set and front lane, the stream of the stage
 // being enqueued, the unit of the persistent kernels' grids and whether stage marks are recorded.

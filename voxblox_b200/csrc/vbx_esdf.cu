@@ -727,43 +727,28 @@ __global__ void k_esdf_clear_tsdf_flag(Tables tab, const uint32_t* __restrict__ 
 
 static inline unsigned int grid_for(uint64_t n, int block) { return (unsigned int)((n + block - 1) / block); }
 
-int esdf_destroy(vbx_ctx* c) {
-  void* ptrs[] = {c->tab.esdf, c->frontier[0], c->frontier[1], c->raise_q[0], c->raise_q[1], c->esdf_block_list,
-                  c->esdf_seed_list, c->esdf_seed_val, c->esdf_touched, c->esdf_fe, c->esdf_d_state};
-  for (void* p : ptrs) {
-    if (p) cudaFree(p);
-  }
-  if (c->esdf_h_state) cudaFreeHost(c->esdf_h_state);
-  c->esdf_fe = nullptr;
-  c->esdf_d_state = c->esdf_h_state = nullptr;
-  c->tab.esdf = nullptr;
-  c->frontier[0] = c->frontier[1] = c->raise_q[0] = c->raise_q[1] = c->esdf_block_list = nullptr;
-  c->esdf_seed_list = c->esdf_touched = nullptr;
-  c->esdf_seed_val = nullptr;
-  c->has_esdf = false;
-  return VBX_OK;
-}
-
 int esdf_create(vbx_ctx* c, const vbx_esdf_config* cfg) {
-  if (c->has_esdf) esdf_destroy(c);
+  Holdings& h = c->own_esdf;
+  h.release();  // the previous ESDF, or what a failed call allocated
+  c->has_esdf = false;
   c->ecfg = *cfg;
   const size_t nvox = (size_t)c->tab.max_blocks * c->vox_per_block;
-  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->tab.esdf), nvox * sizeof(EsdfVoxel)));
+  VBX_CUDA(c, h.dev(&c->tab.esdf, nvox));
   // new Block<EsdfVoxel>: distance 0, all flags false, parent 0 (core/voxel.h:18-37)
   VBX_CUDA(c, cudaMemsetAsync(c->tab.esdf, 0, nvox * sizeof(EsdfVoxel), c->stream));
   VBX_CUDA(c, cudaMemsetAsync(c->tab.slot_has_esdf, 0, c->tab.max_blocks, c->stream));
   VBX_CUDA(c, cudaMemsetAsync(c->tab.slot_esdf_updated, 0, c->tab.max_blocks, c->stream));
   c->frontier_cap = std::min<uint64_t>(nvox, 1ull << 25);
   for (int i = 0; i < 2; ++i) {
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->frontier[i]), c->frontier_cap * sizeof(uint32_t)));
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->raise_q[i]), c->frontier_cap * sizeof(uint32_t)));
+    VBX_CUDA(c, h.dev(&c->frontier[i], c->frontier_cap));
+    VBX_CUDA(c, h.dev(&c->raise_q[i], c->frontier_cap));
   }
-  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_block_list), c->tab.max_blocks * sizeof(uint32_t)));
-  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_seed_list), c->frontier_cap * sizeof(uint32_t)));
-  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_seed_val), c->frontier_cap * sizeof(float)));
-  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_touched), c->frontier_cap * sizeof(uint32_t)));
-  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_d_state), sizeof(EsdfState)));
-  VBX_CUDA(c, cudaMallocHost(reinterpret_cast<void**>(&c->esdf_h_state), sizeof(EsdfState)));
+  VBX_CUDA(c, h.dev(&c->esdf_block_list, c->tab.max_blocks));
+  VBX_CUDA(c, h.dev(&c->esdf_seed_list, c->frontier_cap));
+  VBX_CUDA(c, h.dev(&c->esdf_seed_val, c->frontier_cap));
+  VBX_CUDA(c, h.dev(&c->esdf_touched, c->frontier_cap));
+  VBX_CUDA(c, h.dev(&c->esdf_d_state, 1));
+  VBX_CUDA(c, h.host(&c->esdf_h_state, 1));
   int dev = c->device, sms = 0, per_sm_r = 0, per_sm_l = 0;
   VBX_CUDA(c, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   VBX_CUDA(c, cudaFuncSetAttribute(k_esdf_propagate, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -917,8 +902,7 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
   E.cap = (uint32_t)c->frontier_cap;
   Tally tally{c, s, c->profiling};
   if (E.full_euclidean && !c->esdf_fe) {
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->esdf_fe),
-                           (size_t)c->tab.max_blocks * c->vox_per_block * sizeof(unsigned long long)));
+    VBX_CUDA(c, c->own_esdf.dev(&c->esdf_fe, (size_t)c->tab.max_blocks * c->vox_per_block));
   }
   EsdfState* d_state = c->esdf_d_state;
   const EsdfState& h = *c->esdf_h_state;

@@ -305,7 +305,8 @@ int icp_debug_solve(vbx_ctx* c, uint32_t n, int refine_roll_pitch, const float* 
   // one device allocation: h (9), m (9), q (4), w (3) in; r (9), q (4), log (3), exp (4) and valid out, per item
   const size_t nn = n;
   float* d = nullptr;
-  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&d), 46 * nn * sizeof(float)));
+  Holdings scratch;
+  VBX_CUDA(c, scratch.dev(&d, 46 * nn));
   float *dh = d, *dm = dh + 9 * nn, *dq = dm + 9 * nn, *dw = dq + 4 * nn;
   float *dr = dw + 3 * nn, *dqo = dr + 9 * nn, *dl = dqo + 4 * nn, *de = dl + 3 * nn;
   int32_t* dv = reinterpret_cast<int32_t*>(de + 4 * nn);
@@ -313,39 +314,23 @@ int icp_debug_solve(vbx_ctx* c, uint32_t n, int refine_roll_pitch, const float* 
   const float* hin[4] = {h, m, q, w};
   float* din[4] = {dh, dm, dq, dw};
   const size_t width_in[4] = {9, 9, 4, 3};
-  cudaError_t e = cudaSuccess;
-  for (int k = 0; k < 4 && e == cudaSuccess; ++k)
-    e = cudaMemcpyAsync(din[k], hin[k], width_in[k] * nn * sizeof(float), cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) {
-    k_icp_debug_solve<<<(n + 127) / 128, 128, 0, s>>>(n, refine_roll_pitch, std::pow(std::numeric_limits<float>::epsilon(), 0.25f),
-                                                      std::pow(std::numeric_limits<double>::epsilon(), 0.25), dh, dm, dq, dw, dr, dv,
-                                                      dqo, dl, de);
-    ++c->launches;
-    e = cudaGetLastError();
+  for (int k = 0; k < 4; ++k) {
+    VBX_CUDA(c, cudaMemcpyAsync(din[k], hin[k], width_in[k] * nn * sizeof(float), cudaMemcpyHostToDevice, s));
   }
+  k_icp_debug_solve<<<(n + 127) / 128, 128, 0, s>>>(n, refine_roll_pitch, std::pow(std::numeric_limits<float>::epsilon(), 0.25f),
+                                                    std::pow(std::numeric_limits<double>::epsilon(), 0.25), dh, dm, dq, dw, dr, dv,
+                                                    dqo, dl, de);
+  ++c->launches;
+  VBX_CUDA(c, cudaGetLastError());
   float* hout[4] = {r_out, q_out, log_out, exp_out};
   const float* dout[4] = {dr, dqo, dl, de};
   const size_t width_out[4] = {9, 4, 3, 4};
-  for (int k = 0; k < 4 && e == cudaSuccess; ++k)
-    e = cudaMemcpyAsync(hout[k], dout[k], width_out[k] * nn * sizeof(float), cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(valid_out, dv, nn * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  cudaFree(d);
-  return e == cudaSuccess ? VBX_OK : cuda_fail(c, e, "icp_debug_solve");
-}
-
-void icp_destroy(vbx_ctx* c) {
-  if (c->icp_perm_dev) cudaFree(c->icp_perm_dev);
-  if (c->icp_perm_host) cudaFreeHost(c->icp_perm_host);
-  if (c->icp_out_dev) cudaFree(c->icp_out_dev);
-  if (c->icp_out_host) cudaFreeHost(c->icp_out_host);
-  if (c->icp_points_dev) cudaFree(c->icp_points_dev);
-  c->icp_perm_dev = nullptr;
-  c->icp_perm_host = nullptr;
-  c->icp_out_dev = nullptr;
-  c->icp_out_host = nullptr;
-  c->icp_points_dev = nullptr;
-  c->icp_cap = 0;
+  for (int k = 0; k < 4; ++k) {
+    VBX_CUDA(c, cudaMemcpyAsync(hout[k], dout[k], width_out[k] * nn * sizeof(float), cudaMemcpyDeviceToHost, s));
+  }
+  VBX_CUDA(c, cudaMemcpyAsync(valid_out, dv, nn * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaStreamSynchronize(s));
+  return VBX_OK;
 }
 
 int icp_run(vbx_ctx* c, const vbx_icp_config* cfg, const float* points, int on_device, uint64_t n, const float q[4],
@@ -356,13 +341,15 @@ int icp_run(vbx_ctx* c, const vbx_icp_config* cfg, const float* points, int on_d
   const size_t smem = ((size_t)cfg->num_threads * cfg->mini_batch_size * kIcpRec + (size_t)cfg->num_threads * 21) * sizeof(float);
   if (smem > 200 * 1024) return fail(c, VBX_E_CAPACITY, "icp: num_threads * mini_batch_size too large for shared memory");
   if (n > c->icp_cap || !c->icp_out_dev) {
-    icp_destroy(c);
+    Holdings& h = c->own_icp;
+    h.release();
+    c->icp_cap = 0;
     const uint64_t cap = std::max<uint64_t>(n, 1024);
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->icp_perm_dev), cap * sizeof(uint32_t)));
-    VBX_CUDA(c, cudaHostAlloc(reinterpret_cast<void**>(&c->icp_perm_host), cap * sizeof(uint32_t), cudaHostAllocDefault));
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->icp_points_dev), cap * 3 * sizeof(float)));
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->icp_out_dev), 16 * sizeof(float)));
-    VBX_CUDA(c, cudaHostAlloc(reinterpret_cast<void**>(&c->icp_out_host), 16 * sizeof(float), cudaHostAllocDefault));
+    VBX_CUDA(c, h.dev(&c->icp_perm_dev, cap));
+    VBX_CUDA(c, h.host(&c->icp_perm_host, cap));
+    VBX_CUDA(c, h.dev(&c->icp_points_dev, cap * 3));
+    VBX_CUDA(c, h.dev(&c->icp_out_dev, 16));
+    VBX_CUDA(c, h.host(&c->icp_out_host, 16));
     c->icp_cap = cap;
   }
   cudaStream_t s = c->stream;

@@ -292,21 +292,6 @@ __global__ void k_mesh_clear_flag(Tables tab, const uint32_t* __restrict__ slots
 
 static inline unsigned int grid_for(uint64_t n, int block) { return (unsigned int)((n + block - 1) / block); }
 
-static void mesh_free(vbx_ctx* c) {
-  void* ptrs[] = {c->mesh_slots, c->mesh_cube_off, c->mesh_block_nv, c->mesh_first, c->mesh_vertices, c->mesh_normals,
-                  c->mesh_colors};
-  for (void* p : ptrs) {
-    if (p) cudaFree(p);
-  }
-  c->mesh_slots = c->mesh_block_nv = c->mesh_colors = nullptr;
-  c->mesh_cube_off = nullptr;
-  c->mesh_first = nullptr;
-  c->mesh_vertices = c->mesh_normals = nullptr;
-  c->mesh_cap_blocks = c->mesh_cap_vertices = 0;
-}
-
-void mesh_destroy(vbx_ctx* c) { mesh_free(c); }
-
 // MeshIntegrator::generateMesh(only_mesh_updated_blocks, clear_updated_flag), mesh_integrator.h:132-160
 int mesh_generate(vbx_ctx* c, const vbx_mesh_config* cfg, int only_updated, int clear_flag, uint64_t* n_blocks_out,
                   uint64_t* n_vertices_out) {
@@ -326,18 +311,13 @@ int mesh_generate(vbx_ctx* c, const vbx_mesh_config* cfg, int only_updated, int 
   const uint32_t nb = (uint32_t)items.size();
   if (nb > c->mesh_cap_blocks) {
     const uint64_t want = std::max<uint64_t>(2ull * nb, 256);
-    void* old[] = {c->mesh_slots, c->mesh_cube_off, c->mesh_block_nv, c->mesh_first};
-    for (void* p : old) {
-      if (p) cudaFree(p);
-    }
-    c->mesh_slots = c->mesh_block_nv = nullptr;
-    c->mesh_cube_off = nullptr;
-    c->mesh_first = nullptr;
+    Holdings& h = c->own_mesh_blocks;
+    h.release();
     c->mesh_cap_blocks = 0;
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->mesh_slots), want * sizeof(uint32_t)));
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->mesh_cube_off), want * c->vox_per_block * sizeof(uint16_t)));
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->mesh_block_nv), want * sizeof(uint32_t)));
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->mesh_first), (want + 1) * sizeof(unsigned long long)));
+    VBX_CUDA(c, h.dev(&c->mesh_slots, want));
+    VBX_CUDA(c, h.dev(&c->mesh_cube_off, want * c->vox_per_block));
+    VBX_CUDA(c, h.dev(&c->mesh_block_nv, want));
+    VBX_CUDA(c, h.dev(&c->mesh_first, want + 1));
     c->mesh_cap_blocks = want;
   }
   std::vector<uint32_t> slots(nb);
@@ -377,16 +357,12 @@ int mesh_generate(vbx_ctx* c, const vbx_mesh_config* cfg, int only_updated, int 
   const uint64_t total = c->mesh_first_host[nb];
   if (total > c->mesh_cap_vertices) {
     const uint64_t want = std::max<uint64_t>(total + total / 2, 1u << 16);
-    void* old[] = {c->mesh_vertices, c->mesh_normals, c->mesh_colors};
-    for (void* p : old) {
-      if (p) cudaFree(p);
-    }
-    c->mesh_vertices = c->mesh_normals = nullptr;
-    c->mesh_colors = nullptr;
+    Holdings& h = c->own_mesh_vertices;
+    h.release();
     c->mesh_cap_vertices = 0;
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->mesh_vertices), want * 3 * sizeof(float)));
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->mesh_normals), want * 3 * sizeof(float)));
-    VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&c->mesh_colors), want * sizeof(uint32_t)));
+    VBX_CUDA(c, h.dev(&c->mesh_vertices, want * 3));
+    VBX_CUDA(c, h.dev(&c->mesh_normals, want * 3));
+    VBX_CUDA(c, h.dev(&c->mesh_colors, want));
     c->mesh_cap_vertices = want;
   }
   uint64_t launches = 1;

@@ -42,6 +42,7 @@
 #include <cstdio>
 #include <cstring>
 #include <numeric>
+#include <utility>
 #include <unordered_map>  // std::__detail::_Prime_rehash_policy: the growth schedule the reference's map follows
 
 #include <cooperative_groups.h>
@@ -2334,9 +2335,9 @@ int create_listed_blocks(vbx_ctx* c, uint8_t new_bits) {
   return VBX_OK;
 }
 
-int alloc_scan_args(vbx_ctx* c, vbx_ctx::ScratchSet& S) {
-  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&S.d_args), sizeof(ScanArgs)));
-  VBX_CUDA(c, cudaMallocHost(reinterpret_cast<void**>(&S.h_args), sizeof(ScanArgs)));
+int alloc_scan_args(vbx_ctx* c, Holdings& h, vbx_ctx::ScratchSet& S) {
+  VBX_CUDA(c, h.dev(&S.d_args, 1));
+  VBX_CUDA(c, h.host(&S.h_args, 1));
   return VBX_OK;
 }
 
@@ -2627,6 +2628,9 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
   VBX_CUDA(c, cudaStreamBeginCapture(o, cudaStreamCaptureModeThreadLocal));
   int rc = enqueue();
   cudaGraph_t g = nullptr;
+  cudaGraphExec_t x = nullptr;
+  Holdings pending;  // the graph and its exec until they are complete and handed to the context
+  pending.graph(&g, &x);
   const cudaError_t e = cudaStreamEndCapture(o, &g);
   if (rc == VBX_OK && e != cudaSuccess) rc = cuda_fail(c, e, "cudaStreamEndCapture");
   // Per-node stage priorities (apply > walk > sort > front, as the streams of the unpipelined stages had)
@@ -2676,7 +2680,6 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
       rc = fail(c, VBX_E_CUDA, "captured scan graph: sort / bundle order node not found");
     }
   }
-  cudaGraphExec_t x = nullptr;
   if (rc == VBX_OK) {
     const cudaError_t ei = cudaGraphInstantiateWithFlags(&x, g, cudaGraphInstantiateFlagUseNodePriority);
     if (ei != cudaSuccess) rc = cuda_fail(c, ei, "cudaGraphInstantiateWithFlags");
@@ -2686,13 +2689,10 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
     const cudaError_t eu = cudaGraphUpload(x, o);
     if (eu != cudaSuccess) rc = cuda_fail(c, eu, "cudaGraphUpload");
   }
-  if (rc != VBX_OK) {
-    if (x) cudaGraphExecDestroy(x);
-    if (g) cudaGraphDestroy(g);
-    return rc;
-  }
-  G.graph = g;
-  G.exec = x;
+  if (rc != VBX_OK) return rc;
+  G.graph = std::exchange(g, nullptr);
+  G.exec = std::exchange(x, nullptr);
+  c->own_async.graph(&G.graph, &G.exec);
   G.launches = launches;
   G.point_sort = point_sort;
   G.point_grid = pp.gridDim.x;
@@ -2979,7 +2979,8 @@ int debug_apply(vbx_ctx* c, const int32_t* idx3, uint32_t nb, uint64_t n, const 
   const size_t n4 = (size_t)n * 4;
   char* buf = nullptr;
   const size_t bytes = (size_t)nb * 8 + 5 * n4 + 4;
-  VBX_CUDA(c, cudaMalloc(reinterpret_cast<void**>(&buf), bytes));
+  Holdings scratch;
+  VBX_CUDA(c, scratch.dev(&buf, bytes));
   uint64_t* d_bkeys = reinterpret_cast<uint64_t*>(buf);
   uint32_t* d_block = reinterpret_cast<uint32_t*>(buf + (size_t)nb * 8);
   uint32_t* d_voxel = d_block + n;
@@ -2987,46 +2988,41 @@ int debug_apply(vbx_ctx* c, const int32_t* idx3, uint32_t nb, uint64_t n, const 
   float* d_w = d_sdf + n;
   uint32_t* d_col = reinterpret_cast<uint32_t*>(d_w + n);
   uint32_t* d_bad = d_col + n;
-  auto run = [&]() -> int {
-    VBX_CUDA(c, cudaMemcpyAsync(d_bkeys, bkeys.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, s));
-    VBX_CUDA(c, cudaMemcpyAsync(d_block, rec_block, n4, cudaMemcpyHostToDevice, s));
-    VBX_CUDA(c, cudaMemcpyAsync(d_voxel, rec_voxel, n4, cudaMemcpyHostToDevice, s));
-    VBX_CUDA(c, cudaMemcpyAsync(d_sdf, sdf, n4, cudaMemcpyHostToDevice, s));
-    VBX_CUDA(c, cudaMemcpyAsync(d_w, w, n4, cudaMemcpyHostToDevice, s));
-    VBX_CUDA(c, cudaMemcpyAsync(d_col, rgba, n4, cudaMemcpyHostToDevice, s));
-    VBX_CUDA(c, cudaMemsetAsync(d_bad, 0, 4, s));
-    ScanParams P;
-    const float q[4] = {1.f, 0.f, 0.f, 0.f}, t[3] = {0.f, 0.f, 0.f};
-    fill_params(c, VBX_SIMPLE, q, t, 0, 0, P);
-    ScanArgs a;
-    fill_args(c, P, nullptr, nullptr, &a);
-    a.count_paths = 1u;
-    if (int rc = upload_args(c, x, a)) return rc;
-    VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), s));
-    VBX_CUDA(c, cudaMemsetAsync(S.sort_plan1, 0, sizeof(SortPlan), s));  // (sort_and_apply expects it cleared)
-    const uint64_t m = std::max<uint64_t>(n, nb);
-    if (m) {
-      k_debug_apply_setup<<<grid_for(m, 256), 256, 0, s>>>(scan_tables(c, S), d_bkeys, nb, d_block, d_voxel, n, c->L,
-                                                           S.ckeys[0], S.cvals[0], S.d_state, d_bad);
-    }
-    uint32_t bad = 0;
-    VBX_CUDA(c, cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
-    VBX_CUDA(c, cudaStreamSynchronize(s));
-    if (bad) return fail(c, VBX_E_INVALID, "debug_apply: a block is not in the TSDF layer");
-    Tally tally{c, s, x.marks};
-    const GivenRecords given{d_sdf, d_w, d_col};
-    if (int rc = sort_and_apply(c, x, tally, nullptr, &given)) return rc;
-    VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
-    VBX_CUDA(c, cudaStreamSynchronize(s));
-    VBX_CUDA(c, cudaGetLastError());
-    if (int rc = check_state_errors(c, *S.h_state)) return rc;
-    report_apply_paths(c, *S.h_state);
-    if (paths) std::memcpy(paths, c->apply_paths, sizeof(c->apply_paths));
-    return VBX_OK;
-  };
-  const int rc = run();
-  cudaFree(buf);
-  return rc;
+  VBX_CUDA(c, cudaMemcpyAsync(d_bkeys, bkeys.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, s));
+  VBX_CUDA(c, cudaMemcpyAsync(d_block, rec_block, n4, cudaMemcpyHostToDevice, s));
+  VBX_CUDA(c, cudaMemcpyAsync(d_voxel, rec_voxel, n4, cudaMemcpyHostToDevice, s));
+  VBX_CUDA(c, cudaMemcpyAsync(d_sdf, sdf, n4, cudaMemcpyHostToDevice, s));
+  VBX_CUDA(c, cudaMemcpyAsync(d_w, w, n4, cudaMemcpyHostToDevice, s));
+  VBX_CUDA(c, cudaMemcpyAsync(d_col, rgba, n4, cudaMemcpyHostToDevice, s));
+  VBX_CUDA(c, cudaMemsetAsync(d_bad, 0, 4, s));
+  ScanParams P;
+  const float q[4] = {1.f, 0.f, 0.f, 0.f}, t[3] = {0.f, 0.f, 0.f};
+  fill_params(c, VBX_SIMPLE, q, t, 0, 0, P);
+  ScanArgs a;
+  fill_args(c, P, nullptr, nullptr, &a);
+  a.count_paths = 1u;
+  if (int rc = upload_args(c, x, a)) return rc;
+  VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), s));
+  VBX_CUDA(c, cudaMemsetAsync(S.sort_plan1, 0, sizeof(SortPlan), s));  // (sort_and_apply expects it cleared)
+  const uint64_t m = std::max<uint64_t>(n, nb);
+  if (m) {
+    k_debug_apply_setup<<<grid_for(m, 256), 256, 0, s>>>(scan_tables(c, S), d_bkeys, nb, d_block, d_voxel, n, c->L,
+                                                         S.ckeys[0], S.cvals[0], S.d_state, d_bad);
+  }
+  uint32_t bad = 0;
+  VBX_CUDA(c, cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaStreamSynchronize(s));
+  if (bad) return fail(c, VBX_E_INVALID, "debug_apply: a block is not in the TSDF layer");
+  Tally tally{c, s, x.marks};
+  const GivenRecords given{d_sdf, d_w, d_col};
+  if (int rc = sort_and_apply(c, x, tally, nullptr, &given)) return rc;
+  VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaStreamSynchronize(s));
+  VBX_CUDA(c, cudaGetLastError());
+  if (int rc = check_state_errors(c, *S.h_state)) return rc;
+  report_apply_paths(c, *S.h_state);
+  if (paths) std::memcpy(paths, c->apply_paths, sizeof(c->apply_paths));
+  return VBX_OK;
 }
 
 // exclusive prefix sum of n host uint32 through the engine's scan kernel
