@@ -48,8 +48,6 @@ __global__ void k_rebuild_hash(Tables tab, uint32_t n_blocks) {
   }
 }
 
-static inline unsigned int grid_for(uint64_t n, int block) { return (unsigned int)((n + block - 1) / block); }
-
 // The block transfer kernels take the block number from blockIdx.y, which is capped at 65,535: larger
 // batches are launched in slices of at most that many blocks.
 static constexpr uint64_t kMaxGridY = 65535;
@@ -149,16 +147,16 @@ __global__ void k_scatter_blocks(int layer, int serialized, const uint32_t* __re
 }
 
 static int ensure_staging(vbx_ctx* c, size_t bytes, size_t slots) {
-  if (bytes <= c->mirror_cap_bytes && slots <= c->mirror_cap_slots) return VBX_OK;
-  Holdings& h = c->own_staging;
+  if (bytes <= c->mirror.cap_bytes && slots <= c->mirror.cap_slots) return VBX_OK;
+  Holdings& h = c->mirror.own;
   h.release();
-  c->mirror_cap_bytes = c->mirror_cap_slots = 0;
+  c->mirror.cap_bytes = c->mirror.cap_slots = 0;
   const size_t want_b = std::max<size_t>(2 * bytes, 16u << 20), want_s = std::max<size_t>(2 * slots, 1024);
-  VBX_CUDA(c, h.dev(&c->mirror_dev, want_b));
-  VBX_CUDA(c, h.host(&c->mirror_host, want_b));
-  VBX_CUDA(c, h.dev(&c->mirror_slots, want_s));
-  c->mirror_cap_bytes = want_b;
-  c->mirror_cap_slots = want_s;
+  VBX_CUDA(c, h.dev(&c->mirror.dev, want_b));
+  VBX_CUDA(c, h.host(&c->mirror.host, want_b));
+  VBX_CUDA(c, h.dev(&c->mirror.slots, want_s));
+  c->mirror.cap_bytes = want_b;
+  c->mirror.cap_slots = want_s;
   return VBX_OK;
 }
 
@@ -240,7 +238,7 @@ static int scatter_listed(vbx_ctx* c, int layer, int serialized, const void* src
 int upload_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, const void* voxels,
                   const uint8_t* updated_bits, int serialized) {
   if (m == 0) return VBX_OK;
-  if (layer == VBX_LAYER_ESDF && !c->has_esdf) return fail(c, VBX_E_STATE, "no ESDF layer");
+  if (layer == VBX_LAYER_ESDF && !c->esdf.ready) return fail(c, VBX_E_STATE, "no ESDF layer");
   if (m > c->tab.max_blocks) return fail(c, VBX_E_CAPACITY, "more blocks than the pool holds");
   cudaStream_t s = c->stream;
   std::vector<uint64_t> keys;
@@ -254,13 +252,13 @@ int upload_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, const 
   const size_t bbytes = payload_bytes(c, layer, serialized);
   const uint64_t chunk = std::max<uint64_t>(1, std::min<uint64_t>(listed, (256ull << 20) / bbytes));
   if (int rc = ensure_staging(c, chunk * bbytes + chunk, chunk)) return rc;
-  uint8_t* d_upd = static_cast<uint8_t*>(c->mirror_dev) + chunk * bbytes;
+  uint8_t* d_upd = static_cast<uint8_t*>(c->mirror.dev) + chunk * bbytes;
   for (uint64_t at = 0; at < listed; at += chunk) {
     const uint64_t k = std::min<uint64_t>(chunk, listed - at);
-    VBX_CUDA(c, cudaMemcpyAsync(c->mirror_dev, static_cast<const char*>(voxels) + at * bbytes, k * bbytes,
+    VBX_CUDA(c, cudaMemcpyAsync(c->mirror.dev, static_cast<const char*>(voxels) + at * bbytes, k * bbytes,
                                 cudaMemcpyHostToDevice, s));
     if (updated_bits) VBX_CUDA(c, cudaMemcpyAsync(d_upd, updated_bits + at, k, cudaMemcpyHostToDevice, s));
-    if (int rc = scatter_listed(c, layer, serialized, c->mirror_dev, at, k, updated_bits ? d_upd : nullptr, 0)) return rc;
+    if (int rc = scatter_listed(c, layer, serialized, c->mirror.dev, at, k, updated_bits ? d_upd : nullptr, 0)) return rc;
     VBX_CUDA(c, cudaStreamSynchronize(s));  // the staging buffer is reused by the next chunk
   }
   if (err) return err;
@@ -275,7 +273,7 @@ int upload_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m, const 
 int upload_blocks_device(vbx_ctx* c, int layer, const int32_t* d_idx3, uint64_t m, const void* d_voxels,
                          uint8_t updated_bits) {
   if (m == 0) return VBX_OK;
-  if (layer == VBX_LAYER_ESDF && !c->has_esdf) return fail(c, VBX_E_STATE, "no ESDF layer");
+  if (layer == VBX_LAYER_ESDF && !c->esdf.ready) return fail(c, VBX_E_STATE, "no ESDF layer");
   if (m > c->tab.max_blocks) return fail(c, VBX_E_CAPACITY, "more blocks than the pool holds");
   std::vector<int32_t> idx(3 * m);
   VBX_CUDA(c, cudaMemcpyAsync(idx.data(), d_idx3, 3 * m * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
@@ -304,8 +302,8 @@ int remove_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m);
 // Layer::removeAllBlocks (core/layer.h:164) of ONE layer; the other layer keeps its blocks
 int clear_layer(vbx_ctx* c, int layer) {
   cudaStream_t s = c->stream;
-  if (layer == VBX_LAYER_ESDF && !c->has_esdf) return VBX_OK;
-  if (c->has_esdf && c->n_blocks) {
+  if (layer == VBX_LAYER_ESDF && !c->esdf.ready) return VBX_OK;
+  if (c->esdf.ready && c->n_blocks) {
     // the layers share pool slots: remove this layer's block from every slot (slots that end up
     // empty are given back)
     if (int rc = refresh_host_mirror(c)) return rc;
@@ -318,7 +316,7 @@ int clear_layer(vbx_ctx* c, int layer) {
   c->has_data_keys[1].clear();
   // no ESDF layer: reset the whole map
   const size_t used = (size_t)c->n_blocks * c->vox_per_block;
-  c->esdf_pending_raise = c->esdf_pending_open = 0;
+  c->esdf.pending_raise = c->esdf.pending_open = 0;
   c->maybe_esdf_only = false;
   VBX_CUDA(c, cudaMemsetAsync(c->tab.tsdf, 0, used * sizeof(TsdfVoxel), s));
   VBX_CUDA(c, cudaMemsetAsync(c->tab.hkeys, 0xff, (size_t)c->hcap * sizeof(uint64_t), s));
@@ -382,10 +380,10 @@ int remove_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m) {
     c->has_data_keys[esdf ? 1 : 0].erase(key);
     names_slot = names_slot || c->host_key2slot.count(key);
   }
-  if (!names_slot || (esdf && !c->has_esdf)) return VBX_OK;  // erasing a missing block is a no-op
+  if (!names_slot || (esdf && !c->esdf.ready)) return VBX_OK;  // erasing a missing block is a no-op
   // queue entries of addNewRobotPosition address voxels by slot: they are dropped once the call names an
   // allocated slot, whichever layer holds it
-  c->esdf_pending_raise = c->esdf_pending_open = 0;
+  c->esdf.pending_raise = c->esdf.pending_open = 0;
   std::vector<int32_t> victims(m);
   own.find(idx3, m, victims.data());
   victims.erase(std::remove(victims.begin(), victims.end(), -1), victims.end());
@@ -419,9 +417,9 @@ int remove_blocks(vbx_ctx* c, int layer, const int32_t* idx3, uint64_t m) {
   }
   if (moves.empty()) return VBX_OK;
   if (int rc = ensure_staging(c, moves.size() * sizeof(SlotMove), 0)) return rc;
-  VBX_CUDA(c, cudaMemcpyAsync(c->mirror_dev, moves.data(), moves.size() * sizeof(SlotMove), cudaMemcpyHostToDevice, s));
-  k_compact_pool<<<(unsigned int)moves.size(), 256, 0, s>>>(c->tab, static_cast<const SlotMove*>(c->mirror_dev), n,
-                                                             c->has_esdf ? 1 : 0);
+  VBX_CUDA(c, cudaMemcpyAsync(c->mirror.dev, moves.data(), moves.size() * sizeof(SlotMove), cudaMemcpyHostToDevice, s));
+  k_compact_pool<<<(unsigned int)moves.size(), 256, 0, s>>>(c->tab, static_cast<const SlotMove*>(c->mirror.dev), n,
+                                                             c->esdf.ready ? 1 : 0);
   VBX_CUDA(c, cudaGetLastError());
   VBX_CUDA(c, cudaStreamSynchronize(s));  // (moves lives on this stack frame)
   if (drop.empty()) return VBX_OK;
@@ -439,7 +437,7 @@ int read_layer_slots(vbx_ctx* c, int layer, LayerSlots* v) {
   v->c = c;
   v->flags.assign(n, 0);
   v->member.assign(n, 0);
-  if (n == 0 || (layer == VBX_LAYER_ESDF && !c->has_esdf)) return VBX_OK;
+  if (n == 0 || (layer == VBX_LAYER_ESDF && !c->esdf.ready)) return VBX_OK;
   const bool tsdf = layer == VBX_LAYER_TSDF;
   VBX_CUDA(c, cudaMemcpyAsync(v->flags.data(), tsdf ? c->tab.slot_updated : c->tab.slot_esdf_updated, n,
                               cudaMemcpyDeviceToHost, c->stream));
@@ -549,7 +547,7 @@ int mirror_updated(vbx_ctx* c, int layer, int updated_mask, int clear_mask, int3
     }
     if (updated_bits) updated_bits[i] = view.flags[items[i].slot] & kReportedBits;
   }
-  VBX_CUDA(c, cudaMemcpyAsync(c->mirror_slots, slots.data(), m * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+  VBX_CUDA(c, cudaMemcpyAsync(c->mirror.slots, slots.data(), m * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
   const char* pool = (layer == VBX_LAYER_TSDF) ? reinterpret_cast<const char*>(c->tab.tsdf)
                                                : reinterpret_cast<const char*>(c->tab.esdf);
   if (serialized) {
@@ -558,21 +556,21 @@ int mirror_updated(vbx_ctx* c, int layer, int updated_mask, int clear_mask, int3
       const size_t kb = std::min<size_t>(kMaxGridY, m - b0);
       const dim3 grid(grid_for((uint64_t)tpv * c->vox_per_block, 256), (unsigned int)kb);
       k_serialize_blocks<<<grid, 256, 0, s>>>(
-          layer, reinterpret_cast<const uint32_t*>(pool), c->mirror_slots + b0, (uint32_t)kb, (uint32_t)c->vox_per_block,
-          reinterpret_cast<uint32_t*>(static_cast<char*>(c->mirror_dev) + b0 * bbytes), flags,
+          layer, reinterpret_cast<const uint32_t*>(pool), c->mirror.slots + b0, (uint32_t)kb, (uint32_t)c->vox_per_block,
+          reinterpret_cast<uint32_t*>(static_cast<char*>(c->mirror.dev) + b0 * bbytes), flags,
           (uint8_t)(clear_mask & kMirrorBits));
       VBX_CUDA(c, cudaGetLastError());
     }
   } else if (raw_bytes % 16 == 0) {
-    k_gather_blocks<<<(unsigned int)(m * 8), 256, 0, s>>>(reinterpret_cast<const uint4*>(pool), c->mirror_slots,
+    k_gather_blocks<<<(unsigned int)(m * 8), 256, 0, s>>>(reinterpret_cast<const uint4*>(pool), c->mirror.slots,
                                                            (uint32_t)m, (uint32_t)(raw_bytes / 16),
-                                                           reinterpret_cast<uint4*>(c->mirror_dev), flags,
+                                                           reinterpret_cast<uint4*>(c->mirror.dev), flags,
                                                            (uint8_t)(clear_mask & kMirrorBits));
     VBX_CUDA(c, cudaGetLastError());
   } else {
     k_gather_words<<<grid_for((uint64_t)m * (raw_bytes / 4), 256), 256, 0, s>>>(
-        reinterpret_cast<const uint32_t*>(pool), c->mirror_slots, (uint32_t)m, (uint32_t)(raw_bytes / 4),
-        static_cast<uint32_t*>(c->mirror_dev), flags, (uint8_t)(clear_mask & kMirrorBits));
+        reinterpret_cast<const uint32_t*>(pool), c->mirror.slots, (uint32_t)m, (uint32_t)(raw_bytes / 4),
+        static_cast<uint32_t*>(c->mirror.dev), flags, (uint8_t)(clear_mask & kMirrorBits));
     VBX_CUDA(c, cudaGetLastError());
   }
   // straight into the caller's buffer when it is page-locked (vbx_host_alloc / cudaHostRegister),
@@ -580,11 +578,11 @@ int mirror_updated(vbx_ctx* c, int layer, int updated_mask, int clear_mask, int3
   cudaPointerAttributes attr;
   const bool direct = voxels && cudaPointerGetAttributes(&attr, voxels) == cudaSuccess && attr.type == cudaMemoryTypeHost;
   cudaGetLastError();  // (an unregistered pointer may leave a sticky-free error code behind)
-  void* dst = direct ? voxels : c->mirror_host;
-  VBX_CUDA(c, cudaMemcpyAsync(dst, c->mirror_dev, m * bbytes, cudaMemcpyDeviceToHost, s));
+  void* dst = direct ? voxels : c->mirror.host;
+  VBX_CUDA(c, cudaMemcpyAsync(dst, c->mirror.dev, m * bbytes, cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));
   VBX_CUDA(c, cudaGetLastError());
-  if (!direct && voxels) std::memcpy(voxels, c->mirror_host, m * bbytes);
+  if (!direct && voxels) std::memcpy(voxels, c->mirror.host, m * bbytes);
   return VBX_OK;
 }
 
@@ -610,12 +608,12 @@ int gather_updated_device(vbx_ctx* c, int layer, int updated_mask, int clear_mas
   *n = items.size();
   if (items.empty() || items.size() > cap) return VBX_OK;  // (too small a buffer: nothing copied or cleared)
   const size_t m = items.size();
-  if (m > c->xfer_cap_slots) {
-    c->own_xfer.release();
-    c->xfer_cap_slots = 0;
+  if (m > c->xfer.cap_slots) {
+    c->xfer.own.release();
+    c->xfer.cap_slots = 0;
     const size_t want = std::max<size_t>(2 * m, 1024);
-    VBX_CUDA(c, c->own_xfer.dev(&c->xfer_slots, want));
-    c->xfer_cap_slots = want;
+    VBX_CUDA(c, c->xfer.own.dev(&c->xfer.slots, want));
+    c->xfer.cap_slots = want;
   }
   std::vector<int32_t> idx(3 * m);
   std::vector<uint32_t> slots(m);
@@ -626,19 +624,19 @@ int gather_updated_device(vbx_ctx* c, int layer, int updated_mask, int clear_mas
     idx[3 * i + 2] = items[i].z;
   }
   VBX_CUDA(c, cudaMemcpyAsync(d_idx3, idx.data(), 3 * m * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-  VBX_CUDA(c, cudaMemcpyAsync(c->xfer_slots, slots.data(), m * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+  VBX_CUDA(c, cudaMemcpyAsync(c->xfer.slots, slots.data(), m * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
   uint8_t* flags = (layer == VBX_LAYER_TSDF) ? c->tab.slot_updated : c->tab.slot_esdf_updated;
   const size_t raw_bytes = ((layer == VBX_LAYER_TSDF) ? sizeof(TsdfVoxel) : sizeof(EsdfVoxel)) * c->vox_per_block;
   const char* pool = (layer == VBX_LAYER_TSDF) ? reinterpret_cast<const char*>(c->tab.tsdf)
                                                : reinterpret_cast<const char*>(c->tab.esdf);
   const uint8_t clear = (uint8_t)(clear_mask & kMirrorBits);
   if (raw_bytes % 16 == 0 && reinterpret_cast<uintptr_t>(d_voxels) % 16 == 0) {
-    k_gather_blocks<<<(unsigned int)(m * 8), 256, 0, s>>>(reinterpret_cast<const uint4*>(pool), c->xfer_slots,
+    k_gather_blocks<<<(unsigned int)(m * 8), 256, 0, s>>>(reinterpret_cast<const uint4*>(pool), c->xfer.slots,
                                                            (uint32_t)m, (uint32_t)(raw_bytes / 16),
                                                            static_cast<uint4*>(d_voxels), flags, clear);
   } else {
     k_gather_words<<<grid_for((uint64_t)m * (raw_bytes / 4), 256), 256, 0, s>>>(
-        reinterpret_cast<const uint32_t*>(pool), c->xfer_slots, (uint32_t)m, (uint32_t)(raw_bytes / 4),
+        reinterpret_cast<const uint32_t*>(pool), c->xfer.slots, (uint32_t)m, (uint32_t)(raw_bytes / 4),
         static_cast<uint32_t*>(d_voxels), flags, clear);
   }
   VBX_CUDA(c, cudaGetLastError());

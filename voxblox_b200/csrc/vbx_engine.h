@@ -151,7 +151,7 @@ struct Tables {
   uint8_t* slot_esdf_updated;  // [max_blocks] ESDF Block::updated() bits
   uint8_t* slot_has_esdf;      // [max_blocks] 1 once the ESDF layer holds this block
   TsdfVoxel* tsdf;        // [max_blocks << 3L]
-  EsdfVoxel* esdf;        // [max_blocks << 3L] (allocated by vbx_esdf_create)
+  EsdfVoxel* esdf;        // [max_blocks << 3L] (allocated by vbx_esdf_create, held by vbx_ctx::esdf.own)
 };
 
 // A scan's private block table (hand-off set private, beside touched_list).  The ray walk that writes the
@@ -191,6 +191,7 @@ __host__ __device__ inline uint32_t hash64(uint64_t k) {
   k ^= k >> 33;
   return (uint32_t)k;
 }
+inline unsigned int grid_for(uint64_t n, int block) { return (unsigned int)((n + block - 1) / block); }
 
 // The owner of a group of CUDA resources that share one lifetime: the only code that allocates, creates, frees
 // or destroys them.  Each method stores the new handle in the field it is given and records that field's
@@ -275,8 +276,6 @@ struct vbx_ctx {
   // scratch
   uint32_t max_points = 0;
   uint64_t max_updates = 0;
-  bool timeline = false;            // VBX_ASYNC_TIMELINE: the hand-off events carry timestamps
-  cudaEvent_t timeline_ref = nullptr;
   uint32_t bundle_hint = 0;         // bundles (the larger of the two maps) of the most recent Merged scan whose counters reached the host
   uint64_t record_hint = 1u << 20;  // update records of the most recent scan whose count reached the host: sizes the record sort's grid
   uint32_t* order = nullptr;               // [max_points] "sorted" integration order
@@ -301,8 +300,7 @@ struct vbx_ctx {
   // graph per (hand-off set, front lane, kind), captured before its first use.  The sets and lanes are the
   // only owners of per-scan scratch: set 0 / lane 0 (allocated by vbx_create) are the buffers the synchronous
   // calls use, the others are allocated on the first asynchronous submission (alloc_set / alloc_lane).
-  static constexpr int kSets = 16, kLanes = 8;  // upper bounds
-  int sets_in_use = 10, lanes_in_use = 6;  // (tuning aids: VBX_ASYNC_SETS, VBX_ASYNC_LANES)
+  static constexpr int kSets = 16, kLanes = 8;  // upper bounds of pipe.sets_in_use / pipe.lanes_in_use
   enum { kGraphSimple, kGraphMerged, kGraphVariants };
   struct ScanGraph {
     cudaGraph_t graph = nullptr;
@@ -358,7 +356,7 @@ struct vbx_ctx {
     int freespace = 0;
     const float* in_xyz = nullptr;
     const uint8_t* in_rgba = nullptr;
-  } set[kSets];
+  } set[kSets];  // set 0's buffers are held by own_core; every set's stream and events, and the others' buffers, by pipe.own
   struct FrontLane {  // scratch private to one front-half stream
     cudaStream_t stream = nullptr;
     uint64_t* pkeys1 = nullptr;  // the point sort's second key buffer
@@ -372,77 +370,20 @@ struct vbx_ctx {
     cudaStream_t side = nullptr;      // k_bundle_order runs here, beside k_merge
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     cudaEvent_t done = nullptr;  // the lane's last front half
-  } lane[kLanes];
-  bool async_ready = false;
+  } lane[kLanes];  // lane 0's buffers, side stream and fork / join events are held by own_core; the rest by pipe.own
   int prio_lo = 0, prio_hi = 0;  // stream priority range of the device
-  // the streams a scan's graph is captured from (besides the front lane's and the main stream)
-  cudaStream_t stream_e = nullptr;  // block creation: k_back_begin, k_assign
-  cudaStream_t stream_s = nullptr;  // record sort + apply preparation
-  cudaEvent_t cap_ev[8] = {};  // capture-internal edges (fork, front -> walk, walk -> sort, sort -> apply, joins)
-  uint64_t async_seq = 0;
-  uint32_t* d_hold = nullptr;           // device flag: a queued scan must be redone, later scans skip their back half
-  uint64_t async_redone = 0;            // scans redone synchronously since vbx_create (reporting)
-  bool hash_dirty = false;              // an asynchronous scan ran out of pool slots: rebuild the hash at the next drain
-  int deferred_rc = 0;
-  std::string deferred_msg;
-  // incremental device -> host mirror (vbx_mirror_updated): gather staging on both sides
-  void* mirror_dev = nullptr;
-  void* mirror_host = nullptr;  // page-locked
-  uint32_t* mirror_slots = nullptr;
-  size_t mirror_cap_bytes = 0, mirror_cap_slots = 0;
-  // device-to-device block transfer (vbx_gather_updated_device): the gathered blocks' slots, device only
-  uint32_t* xfer_slots = nullptr;
-  size_t xfer_cap_slots = 0;
   // host mirror of slot_key (refreshed lazily)
   std::vector<uint64_t> host_slot_key;
   std::unordered_map<uint64_t, int32_t> host_key2slot;
   // Block::has_data_ (core/block.h:206): never set by the integrators, carried by BlockProto; blocks loaded
   // from a .vxblx file with has_data = true are remembered per layer so that a re-save writes the flag back
   std::unordered_set<uint64_t> has_data_keys[2];
-  // ESDF
-  bool has_esdf = false;
-  vbx_esdf_config ecfg;
-  uint32_t* frontier[2] = {nullptr, nullptr};
-  uint32_t* raise_q[2] = {nullptr, nullptr};
-  uint64_t frontier_cap = 0;
-  uint32_t* esdf_block_list = nullptr;
-  uint32_t* esdf_seed_list = nullptr;
-  float* esdf_seed_val = nullptr;
-  uint32_t* esdf_touched = nullptr;
-  // full-Euclidean mode only (allocated by its first update): every voxel's distance and parent as one 64-bit
-  // word, so that the wavefront lowers both in a single atomicMin (vbx_esdf.cu, fe_pack)
-  unsigned long long* esdf_fe = nullptr;
-  vbx::EsdfState* esdf_d_state = nullptr;
-  vbx::EsdfState* esdf_h_state = nullptr;  // page-locked
-  int esdf_sms = 0, esdf_ctas_wide = 1;
-  uint32_t esdf_pending_raise = 0, esdf_pending_open = 0;  // raise_ / open_ entries queued by addNewRobotPosition
-  bool maybe_esdf_only = false;                            // some slot may carry kSlotNoTsdf
-  // mesher (vbx_mesh.cu): the result of the last vbx_mesh_generate stays on the device until the next one
-  uint32_t* mesh_slots = nullptr;
-  uint16_t* mesh_cube_off = nullptr;
-  uint32_t* mesh_block_nv = nullptr;
-  unsigned long long* mesh_first = nullptr;
-  float* mesh_vertices = nullptr;
-  float* mesh_normals = nullptr;
-  uint32_t* mesh_colors = nullptr;
-  uint64_t mesh_cap_blocks = 0, mesh_cap_vertices = 0, mesh_launches = 0;
-  std::vector<int32_t> mesh_idx;
-  std::vector<uint64_t> mesh_first_host = std::vector<uint64_t>(1, 0);
-  bool mesh_use_color = false;
-  // ICP (vbx_icp.cu): shuffled point order (host page-locked + device), host-cloud staging, result block
-  uint32_t* icp_perm_dev = nullptr;
-  uint32_t* icp_perm_host = nullptr;
-  float* icp_points_dev = nullptr;
-  float* icp_out_dev = nullptr;
-  float* icp_out_host = nullptr;
-  uint64_t icp_cap = 0;
+  bool maybe_esdf_only = false;  // some slot may carry kSlotNoTsdf
   // reporting
   uint64_t counters[16] = {0};
   uint64_t apply_paths[16] = {0};  // ScanState::apply_paths of the last call whose status reached the host
   bool count_apply_paths = false;  // k_apply counts its paths (vbx_debug_count_apply_paths; vbx_debug_apply always does)
   bool serial_fast = false;        // Fast calls walk their rays on one thread, in rank order (vbx_debug_serial_fast)
-  uint64_t async_wait_ns = 0, async_submit_ns = 0;  // host time of vbx_tsdf_integrate_async: waiting for a hand-off set / enqueueing
-  uint64_t esdf_counters[16] = {0};
   float last_ms = 0.f;
   uint64_t launches = 0;
   cudaEvent_t tev0 = nullptr, tev1 = nullptr;  // vbx_timer_*
@@ -451,17 +392,90 @@ struct vbx_ctx {
   double stage_ms[16] = {0};
   uint64_t stage_calls[16] = {0};
   std::string err;
-  // The owners of the fields above, one per lifetime.  Declared last, so that they are destroyed first,
-  // while every field they null is still alive; vbx_destroy synchronises the streams before.
-  vbx::Holdings own_core;          // vbx_create: the map, the Fast sets, set 0 / lane 0 buffers, main streams and events
-  vbx::Holdings own_async;         // ensure_async: every set's and lane's streams and events, the buffers of sets / lanes
-                                   // 1 and up, stream_e / stream_s / cap_ev, the timeline events; the captured scan graphs
-  vbx::Holdings own_esdf;          // esdf_create, and esdf_fe
-  vbx::Holdings own_mesh_blocks;   // mesh_generate's per-block buffers
-  vbx::Holdings own_mesh_vertices;  // ... and its vertex buffers
-  vbx::Holdings own_icp;           // icp_run's buffers
-  vbx::Holdings own_staging;       // mirror_dev / mirror_host / mirror_slots
-  vbx::Holdings own_xfer;          // xfer_slots
+  // Every owner is declared after the fields it holds, so that it is destroyed first and nulls them while they
+  // are alive (vbx_destroy synchronises the streams before).  own_core holds the fields above.
+  vbx::Holdings own_core;  // vbx_create: the map, the Fast sets, set 0 / lane 0 buffers, main streams and events
+  // The structs below are destroyed in reverse order, all before own_core: pipe's graphs use lane 0's events.
+  // The asynchronous pipeline (ensure_async, integrate_async, capture_scan, drain_async)
+  struct Pipeline {
+    bool ready = false;
+    int sets_in_use = 10, lanes_in_use = 6;  // (tuning aids: VBX_ASYNC_SETS, VBX_ASYNC_LANES)
+    // the streams a scan's graph is captured from (besides the front lane's and the main stream)
+    cudaStream_t stream_e = nullptr;  // block creation: k_back_begin, k_assign
+    cudaStream_t stream_s = nullptr;  // record sort + apply preparation
+    cudaEvent_t cap_ev[8] = {};  // capture-internal edges (fork, front -> walk, walk -> sort, sort -> apply, joins)
+    uint64_t seq = 0;
+    uint32_t* d_hold = nullptr;  // device flag: a queued scan must be redone, later scans skip their back half
+    uint64_t redone = 0;         // scans redone synchronously since vbx_create (reporting)
+    bool hash_dirty = false;     // an asynchronous scan ran out of pool slots: rebuild the hash at the next drain
+    int deferred_rc = 0;
+    std::string deferred_msg;
+    bool timeline = false;  // VBX_ASYNC_TIMELINE: the hand-off events carry timestamps
+    cudaEvent_t timeline_ref = nullptr;
+    uint64_t wait_ns = 0, submit_ns = 0;  // host time of vbx_tsdf_integrate_async: waiting for a hand-off set / enqueueing
+    vbx::Holdings own;  // also set[] / lane[] (see there) and the captured scan graphs
+  } pipe;
+  // ESDF (vbx_esdf.cu)
+  struct Esdf {
+    bool ready = false;  // vbx_esdf_create succeeded
+    vbx_esdf_config cfg;
+    uint32_t* frontier[2] = {nullptr, nullptr};
+    uint32_t* raise_q[2] = {nullptr, nullptr};
+    uint64_t frontier_cap = 0;
+    uint32_t* block_list = nullptr;
+    uint32_t* seed_list = nullptr;
+    float* seed_val = nullptr;
+    uint32_t* touched = nullptr;
+    // full-Euclidean mode only (allocated by its first update): every voxel's distance and parent as one 64-bit
+    // word, so that the wavefront lowers both in a single atomicMin (vbx_esdf.cu, fe_pack)
+    unsigned long long* fe = nullptr;
+    vbx::EsdfState* d_state = nullptr;
+    vbx::EsdfState* h_state = nullptr;  // page-locked
+    int sms = 0, ctas_wide = 1;
+    uint32_t pending_raise = 0, pending_open = 0;  // raise_ / open_ entries queued by addNewRobotPosition
+    uint64_t counters[16] = {0};
+    vbx::Holdings own;  // also tab.esdf
+  } esdf;
+  // mesher (vbx_mesh.cu): the result of the last vbx_mesh_generate stays on the device until the next one
+  struct Mesh {
+    uint32_t* slots = nullptr;
+    uint16_t* cube_off = nullptr;
+    uint32_t* block_nv = nullptr;
+    unsigned long long* first = nullptr;
+    float* vertices = nullptr;
+    float* normals = nullptr;
+    uint32_t* colors = nullptr;
+    uint64_t cap_blocks = 0, cap_vertices = 0;
+    std::vector<int32_t> idx;
+    std::vector<uint64_t> first_host = std::vector<uint64_t>(1, 0);
+    bool use_color = false;
+    vbx::Holdings own_blocks;    // the per-block buffers
+    vbx::Holdings own_vertices;  // the vertex buffers
+  } mesh;
+  // ICP (vbx_icp.cu): shuffled point order (host page-locked + device), host-cloud staging, result block
+  struct Icp {
+    uint32_t* perm_dev = nullptr;
+    uint32_t* perm_host = nullptr;
+    float* points_dev = nullptr;
+    float* out_dev = nullptr;
+    float* out_host = nullptr;
+    uint64_t cap = 0;
+    vbx::Holdings own;
+  } icp;
+  // incremental device -> host mirror (vbx_mirror_updated): gather staging on both sides
+  struct Mirror {
+    void* dev = nullptr;
+    void* host = nullptr;  // page-locked
+    uint32_t* slots = nullptr;
+    size_t cap_bytes = 0, cap_slots = 0;
+    vbx::Holdings own;
+  } mirror;
+  // device-to-device block transfer (vbx_gather_updated_device): the gathered blocks' slots, device only
+  struct Xfer {
+    uint32_t* slots = nullptr;
+    size_t cap_slots = 0;
+    vbx::Holdings own;
+  } xfer;
 };
 
 namespace vbx {

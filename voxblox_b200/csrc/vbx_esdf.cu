@@ -428,7 +428,7 @@ __global__ void k_esdf_raise(EsdfParams E, Tables tab, uint32_t* raise_a, uint32
 
 // Full-Euclidean mode: the step a source propagates is computed from its parent vector
 // (voxel_size * (|parent - dir| - |parent|), cc:414-426), so a voxel's distance and parent must change
-// together.  During the wavefront both live in one 64-bit word per voxel (vbx_ctx::esdf_fe):
+// together.  During the wavefront both live in one 64-bit word per voxel (vbx_ctx::esdf.fe):
 //   bits 63..32  the distance's bit pattern as a signed int (the order atomicMin uses, see the top of the file)
 //   bits 31..0   the parent, each component + 512 in 10 bits (x low)
 // so a signed 64-bit atomicMin lowers distance and parent as one unit (equal distances: the smaller parent
@@ -725,30 +725,28 @@ __global__ void k_esdf_clear_tsdf_flag(Tables tab, const uint32_t* __restrict__ 
   tab.slot_updated[block_list[i]] &= (uint8_t)~VBX_UPDATED_ESDF;  // cc:113-121
 }
 
-static inline unsigned int grid_for(uint64_t n, int block) { return (unsigned int)((n + block - 1) / block); }
-
 int esdf_create(vbx_ctx* c, const vbx_esdf_config* cfg) {
-  Holdings& h = c->own_esdf;
+  Holdings& h = c->esdf.own;
   h.release();  // the previous ESDF, or what a failed call allocated
-  c->has_esdf = false;
-  c->ecfg = *cfg;
+  c->esdf.ready = false;
+  c->esdf.cfg = *cfg;
   const size_t nvox = (size_t)c->tab.max_blocks * c->vox_per_block;
   VBX_CUDA(c, h.dev(&c->tab.esdf, nvox));
   // new Block<EsdfVoxel>: distance 0, all flags false, parent 0 (core/voxel.h:18-37)
   VBX_CUDA(c, cudaMemsetAsync(c->tab.esdf, 0, nvox * sizeof(EsdfVoxel), c->stream));
   VBX_CUDA(c, cudaMemsetAsync(c->tab.slot_has_esdf, 0, c->tab.max_blocks, c->stream));
   VBX_CUDA(c, cudaMemsetAsync(c->tab.slot_esdf_updated, 0, c->tab.max_blocks, c->stream));
-  c->frontier_cap = std::min<uint64_t>(nvox, 1ull << 25);
+  c->esdf.frontier_cap = std::min<uint64_t>(nvox, 1ull << 25);
   for (int i = 0; i < 2; ++i) {
-    VBX_CUDA(c, h.dev(&c->frontier[i], c->frontier_cap));
-    VBX_CUDA(c, h.dev(&c->raise_q[i], c->frontier_cap));
+    VBX_CUDA(c, h.dev(&c->esdf.frontier[i], c->esdf.frontier_cap));
+    VBX_CUDA(c, h.dev(&c->esdf.raise_q[i], c->esdf.frontier_cap));
   }
-  VBX_CUDA(c, h.dev(&c->esdf_block_list, c->tab.max_blocks));
-  VBX_CUDA(c, h.dev(&c->esdf_seed_list, c->frontier_cap));
-  VBX_CUDA(c, h.dev(&c->esdf_seed_val, c->frontier_cap));
-  VBX_CUDA(c, h.dev(&c->esdf_touched, c->frontier_cap));
-  VBX_CUDA(c, h.dev(&c->esdf_d_state, 1));
-  VBX_CUDA(c, h.host(&c->esdf_h_state, 1));
+  VBX_CUDA(c, h.dev(&c->esdf.block_list, c->tab.max_blocks));
+  VBX_CUDA(c, h.dev(&c->esdf.seed_list, c->esdf.frontier_cap));
+  VBX_CUDA(c, h.dev(&c->esdf.seed_val, c->esdf.frontier_cap));
+  VBX_CUDA(c, h.dev(&c->esdf.touched, c->esdf.frontier_cap));
+  VBX_CUDA(c, h.dev(&c->esdf.d_state, 1));
+  VBX_CUDA(c, h.host(&c->esdf.h_state, 1));
   int dev = c->device, sms = 0, per_sm_r = 0, per_sm_l = 0;
   VBX_CUDA(c, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   VBX_CUDA(c, cudaFuncSetAttribute(k_esdf_propagate, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -759,10 +757,10 @@ int esdf_create(vbx_ctx* c, const vbx_esdf_config* cfg) {
   // barrier cost (which grows with the number of CTAs) matters more than raw parallelism
   // (measured on the 640x480 workload: 0.45 ms per update with one CTA per SM, 0.52 ms with four);
   // updates over many blocks (batch mode, LiDAR) get the wider grid, see esdf_run
-  c->esdf_sms = sms;
-  c->esdf_ctas_wide = std::max(1, std::min(std::min(per_sm_r, per_sm_l), 4));
+  c->esdf.sms = sms;
+  c->esdf.ctas_wide = std::max(1, std::min(std::min(per_sm_r, per_sm_l), 4));
   VBX_CUDA(c, cudaStreamSynchronize(c->stream));
-  c->has_esdf = true;
+  c->esdf.ready = true;
   return VBX_OK;
 }
 
@@ -771,15 +769,15 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
 
 // EsdfIntegrator::clear(), esdf_integrator.h:135-140: forget the work addNewRobotPosition queued
 int esdf_clear_state(vbx_ctx* c) {
-  c->esdf_pending_raise = c->esdf_pending_open = 0;
+  c->esdf.pending_raise = c->esdf.pending_open = 0;
   return keep_flag_bits(c, c->tab.slot_esdf_updated, (uint8_t)~kEsdfPending);
 }
 
 // EsdfIntegrator::addNewRobotPosition(position), esdf_integrator.cc:25-92
 int esdf_add_robot_position(vbx_ctx* c, const float p[3]) {
   cudaStream_t s = c->stream;
-  const vbx_esdf_config& cfg = c->ecfg;
-  std::memset(c->esdf_counters, 0, sizeof(c->esdf_counters));
+  const vbx_esdf_config& cfg = c->esdf.cfg;
+  std::memset(c->esdf.counters, 0, sizeof(c->esdf.counters));
   Tally tally{c, s, false};
   const float radii[2] = {cfg.clear_sphere_radius, cfg.occupied_sphere_radius};
   SphereParams S[2];
@@ -798,19 +796,19 @@ int esdf_add_robot_position(vbx_ctx* c, const float p[3]) {
     S[k].default_distance = cfg.default_distance_m;
     S[k].L = c->L;
     S[k].outer = k;
-    S[k].cap = (uint32_t)c->frontier_cap;
+    S[k].cap = (uint32_t)c->esdf.frontier_cap;
   }
   // the per-axis lists ride in the seed-value scratch (floats; frontier_cap >> 1300 entries)
-  float* d_xs[2] = {c->esdf_seed_val, c->esdf_seed_val + xs[0].size()};
+  float* d_xs[2] = {c->esdf.seed_val, c->esdf.seed_val + xs[0].size()};
   // block creation: hand-off set 0's block table and status block, as for an upload
   const vbx_ctx::ScratchSet& set0 = c->set[0];
   ScanState* d_state = set0.d_state;
   // the sphere's voxels, queue appends and counters
-  EsdfState* d_es = c->esdf_d_state;
+  EsdfState* d_es = c->esdf.d_state;
   VBX_CUDA(c, cudaEventRecord(c->ev0, s));
   VBX_CUDA(c, cudaMemsetAsync(d_state, 0, sizeof(ScanState), s));
   VBX_CUDA(c, cudaMemsetAsync(d_es, 0, sizeof(EsdfState), s));
-  k_esdf_set_pending<<<1, 1, 0, s>>>(d_es, c->esdf_pending_raise, c->esdf_pending_open);
+  k_esdf_set_pending<<<1, 1, 0, s>>>(d_es, c->esdf.pending_raise, c->esdf.pending_open);
   ++tally.launches;
   for (int k = 0; k < 2; ++k) {
     if (S[k].n == 0) continue;
@@ -825,30 +823,30 @@ int esdf_add_robot_position(vbx_ctx* c, const float p[3]) {
   for (int k = 0; k < 2; ++k) {
     if (S[k].n == 0) continue;
     const uint64_t n3 = (uint64_t)S[k].n * S[k].n * S[k].n;
-    k_esdf_sphere_apply<<<grid_for(n3, 256), 256, 0, s>>>(S[k], c->tab, d_xs[k], c->raise_q[0], c->frontier[0], d_es);
+    k_esdf_sphere_apply<<<grid_for(n3, 256), 256, 0, s>>>(S[k], c->tab, d_xs[k], c->esdf.raise_q[0], c->esdf.frontier[0], d_es);
     ++tally.launches;
   }
   VBX_CUDA(c, cudaEventRecord(c->ev1, s));
   VBX_CUDA(c, cudaMemcpyAsync(set0.h_state, d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, s));
-  VBX_CUDA(c, cudaMemcpyAsync(c->esdf_h_state, d_es, sizeof(EsdfState), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(c->esdf.h_state, d_es, sizeof(EsdfState), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));  // (also keeps xs[] alive until the copies are done)
   VBX_CUDA(c, cudaGetLastError());
   VBX_CUDA(c, cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   const ScanState& h = *set0.h_state;
-  const EsdfState& he = *c->esdf_h_state;
+  const EsdfState& he = *c->esdf.h_state;
   c->n_blocks = h.n_blocks;
   if (h.n_new) c->maybe_esdf_only = true;
   if (h.error & (kErrPoolFull | kErrHashFull)) return check_state_errors(c, h);
   if (h.error & kErrCoordRange) return fail(c, VBX_E_INVALID, "robot position sphere outside the +-2^20 block range");
   if (he.error & kEsdfErrQueueFull) return fail(c, VBX_E_CAPACITY, "ESDF wavefront queue capacity exceeded");
-  c->esdf_pending_raise = he.raise_n[0];
-  c->esdf_pending_open = he.frontier_n[0];
-  c->esdf_counters[0] = h.n_new;          // ESDF blocks created
-  c->esdf_counters[1] = he.counts[1];     // voxels set free
-  c->esdf_counters[2] = he.counts[2];     // voxels set occupied
-  c->esdf_counters[4] = he.raise_n[0];    // queued: raise_
-  c->esdf_counters[5] = he.frontier_n[0]; // queued: open_
-  c->esdf_counters[7] = tally.launches;
+  c->esdf.pending_raise = he.raise_n[0];
+  c->esdf.pending_open = he.frontier_n[0];
+  c->esdf.counters[0] = h.n_new;          // ESDF blocks created
+  c->esdf.counters[1] = he.counts[1];     // voxels set free
+  c->esdf.counters[2] = he.counts[2];     // voxels set occupied
+  c->esdf.counters[4] = he.raise_n[0];    // queued: raise_
+  c->esdf.counters[5] = he.frontier_n[0]; // queued: open_
+  c->esdf.counters[7] = tally.launches;
   c->launches += tally.launches;
   return refresh_host_mirror(c);
 }
@@ -878,8 +876,8 @@ int esdf_update_blocks(vbx_ctx* c, const int32_t* idx3, uint64_t m, int incremen
 static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_flag, const uint32_t* listed_slots,
                     uint32_t n_listed) {
   cudaStream_t s = c->stream;
-  std::memset(c->esdf_counters, 0, sizeof(c->esdf_counters));
-  const vbx_esdf_config& cfg = c->ecfg;
+  std::memset(c->esdf.counters, 0, sizeof(c->esdf.counters));
+  const vbx_esdf_config& cfg = c->esdf.cfg;
   EsdfParams E;
   std::memset(&E, 0, sizeof(E));
   E.L = c->L;
@@ -899,13 +897,13 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
   E.d1 = E.u1 * c->voxel_size;
   E.d2 = E.u2 * c->voxel_size;
   E.d3 = E.u3 * c->voxel_size;
-  E.cap = (uint32_t)c->frontier_cap;
+  E.cap = (uint32_t)c->esdf.frontier_cap;
   Tally tally{c, s, c->profiling};
-  if (E.full_euclidean && !c->esdf_fe) {
-    VBX_CUDA(c, c->own_esdf.dev(&c->esdf_fe, (size_t)c->tab.max_blocks * c->vox_per_block));
+  if (E.full_euclidean && !c->esdf.fe) {
+    VBX_CUDA(c, c->esdf.own.dev(&c->esdf.fe, (size_t)c->tab.max_blocks * c->vox_per_block));
   }
-  EsdfState* d_state = c->esdf_d_state;
-  const EsdfState& h = *c->esdf_h_state;
+  EsdfState* d_state = c->esdf.d_state;
+  const EsdfState& h = *c->esdf.h_state;
   VBX_CUDA(c, cudaEventRecord(c->ev0, s));
   tally.begin();
   VBX_CUDA(c, cudaMemsetAsync(d_state, 0, sizeof(EsdfState), s));
@@ -916,16 +914,16 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
   if (batch) {
     // the batch update wipes the ESDF layer (cc:95); queue entries of addNewRobotPosition would
     // point into removed blocks (the reference CHECK-fails on them), so they are dropped
-    c->esdf_pending_raise = c->esdf_pending_open = 0;
+    c->esdf.pending_raise = c->esdf.pending_open = 0;
   }
   // raise_ / open_ entries queued by addNewRobotPosition since the last update (they sit at the
   // head of raise_q[0] / frontier[0]; this call's own entries are appended behind them)
-  const bool pending = c->esdf_pending_raise || c->esdf_pending_open;
+  const bool pending = c->esdf.pending_raise || c->esdf.pending_open;
   if (pending) {
-    k_esdf_set_pending<<<1, 1, 0, s>>>(d_state, c->esdf_pending_raise, c->esdf_pending_open);
+    k_esdf_set_pending<<<1, 1, 0, s>>>(d_state, c->esdf.pending_raise, c->esdf.pending_open);
     ++tally.launches;
   }
-  c->esdf_pending_raise = c->esdf_pending_open = 0;
+  c->esdf.pending_raise = c->esdf.pending_open = 0;
   if (batch) {
     // esdf_layer_->removeAllBlocks() (cc:95): every ESDF block starts from scratch
     const size_t nvox = (size_t)c->n_blocks * c->vox_per_block;
@@ -937,9 +935,9 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
   if (listed_slots) {
     nb = n_listed;
     if (nb > 0) {
-      VBX_CUDA(c, cudaMemcpyAsync(c->esdf_block_list, listed_slots, (size_t)nb * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+      VBX_CUDA(c, cudaMemcpyAsync(c->esdf.block_list, listed_slots, (size_t)nb * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
       VBX_CUDA(c, cudaMemcpyAsync(&d_state->counts[0], &nb, sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-      k_esdf_mark_listed<<<grid_for(nb, 256), 256, 0, s>>>(c->tab, c->esdf_block_list, nb);
+      k_esdf_mark_listed<<<grid_for(nb, 256), 256, 0, s>>>(c->tab, c->esdf.block_list, nb);
       ++tally.launches;
       VBX_CUDA(c, cudaStreamSynchronize(s));  // the two host sources above are stack / vector memory
     }
@@ -947,7 +945,7 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
     // the list and its length (counts[0]) stay on the device: no host round trip in the middle of
     // the call; the launches below are sized for the upper bound (every slot) and the kernels stop at
     // the real count
-    k_esdf_block_list<<<grid_for(c->n_blocks, 256), 256, 0, s>>>(c->tab, c->n_blocks, batch, c->esdf_block_list, d_state);
+    k_esdf_block_list<<<grid_for(c->n_blocks, 256), 256, 0, s>>>(c->tab, c->n_blocks, batch, c->esdf.block_list, d_state);
     ++tally.launches;
     nb = c->n_blocks;
   }
@@ -956,48 +954,48 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
       // one thread block per voxel block, both slabs staged by the TMA
       const size_t slab_bytes = (size_t)c->vox_per_block * (sizeof(TsdfVoxel) + sizeof(EsdfVoxel));
       k_esdf_propagate<<<nb, (unsigned int)std::max<uint32_t>(32u, std::min<uint32_t>(1024u, c->vox_per_block)), slab_bytes, s>>>(
-          E, c->tab, c->esdf_block_list, nb, c->frontier[0], c->raise_q[0], c->esdf_seed_list, d_state);
+          E, c->tab, c->esdf.block_list, nb, c->esdf.frontier[0], c->esdf.raise_q[0], c->esdf.seed_list, d_state);
       ++tally.launches;
     }
     if (nb > 0 && incremental) {
       const unsigned int g = c->grid_sms * 8;
-      k_esdf_seed<<<g, 256, 0, s>>>(E, c->tab, c->esdf_seed_list, c->frontier[0], c->esdf_seed_val, d_state);
+      k_esdf_seed<<<g, 256, 0, s>>>(E, c->tab, c->esdf.seed_list, c->esdf.frontier[0], c->esdf.seed_val, d_state);
       ++tally.launches;
-      k_esdf_seed_commit<<<g, 256, 0, s>>>(E, c->tab, c->esdf_seed_list, c->esdf_seed_val, d_state);
+      k_esdf_seed_commit<<<g, 256, 0, s>>>(E, c->tab, c->esdf.seed_list, c->esdf.seed_val, d_state);
       ++tally.launches;
     }
     tally.mark(kStageEsdfPropagate);
     // the persistent grid: one CTA per SM for small incremental updates, the wider grid otherwise (esdf_create)
-    int per_sm = (nb <= 256 && !pending) ? 1 : c->esdf_ctas_wide;
-    if (const char* e = std::getenv("VBX_ESDF_CTAS")) per_sm = std::max(1, std::min(std::atoi(e), c->esdf_ctas_wide));  // (tuning aid)
-    const unsigned int grid = (unsigned int)(c->esdf_sms * per_sm);
+    int per_sm = (nb <= 256 && !pending) ? 1 : c->esdf.ctas_wide;
+    if (const char* e = std::getenv("VBX_ESDF_CTAS")) per_sm = std::max(1, std::min(std::atoi(e), c->esdf.ctas_wide));  // (tuning aid)
+    const unsigned int grid = (unsigned int)(c->esdf.sms * per_sm);
     {
-      void* args[] = {&E, &c->tab, &c->raise_q[0], &c->raise_q[1], &c->frontier[0], &d_state};
+      void* args[] = {&E, &c->tab, &c->esdf.raise_q[0], &c->esdf.raise_q[1], &c->esdf.frontier[0], &d_state};
       VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_esdf_raise, dim3(grid), dim3(256), args, 0, s));
       ++tally.launches;
     }
     tally.mark(kStageEsdfRaise);
     long long* fe = nullptr;
     if (E.full_euclidean) {
-      fe = reinterpret_cast<long long*>(c->esdf_fe);
+      fe = reinterpret_cast<long long*>(c->esdf.fe);
       k_esdf_fe_pack<<<c->grid_sms * 8, 256, 0, s>>>(c->tab, (uint64_t)c->n_blocks * c->vox_per_block, fe, d_state);
       ++tally.launches;
     }
     {
-      void* args[] = {&E, &c->tab, &c->frontier[0], &c->frontier[1], &c->esdf_touched, &fe, &d_state};
+      void* args[] = {&E, &c->tab, &c->esdf.frontier[0], &c->esdf.frontier[1], &c->esdf.touched, &fe, &d_state};
       VBX_CUDA(c, cudaLaunchCooperativeKernel((void*)k_esdf_lower, dim3(grid), dim3(256), args, 0, s));
       ++tally.launches;
     }
-    k_esdf_parents<<<c->grid_sms * 8, 256, 0, s>>>(E, c->tab, c->esdf_touched, fe, d_state);
+    k_esdf_parents<<<c->grid_sms * 8, 256, 0, s>>>(E, c->tab, c->esdf.touched, fe, d_state);
     ++tally.launches;
     tally.mark(kStageEsdfLower);
     if (nb > 0 && !batch && clear_updated_flag) {
-      k_esdf_clear_tsdf_flag<<<grid_for(nb, 256), 256, 0, s>>>(c->tab, c->esdf_block_list, d_state);
+      k_esdf_clear_tsdf_flag<<<grid_for(nb, 256), 256, 0, s>>>(c->tab, c->esdf.block_list, d_state);
       ++tally.launches;
     }
   }
   VBX_CUDA(c, cudaEventRecord(c->ev1, s));
-  VBX_CUDA(c, cudaMemcpyAsync(c->esdf_h_state, d_state, sizeof(EsdfState), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(c->esdf.h_state, d_state, sizeof(EsdfState), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));
   VBX_CUDA(c, cudaGetLastError());
   VBX_CUDA(c, cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
@@ -1006,8 +1004,8 @@ static int esdf_run(vbx_ctx* c, int batch, int incremental, int clear_updated_fl
   if (h.error & kEsdfErrParentRange) {
     return fail(c, VBX_E_CAPACITY, "full-Euclidean ESDF: a parent vector component left [-512, 511] voxels");
   }
-  for (int i = 0; i < 7; ++i) c->esdf_counters[i] = h.counts[i];
-  c->esdf_counters[7] = tally.launches;
+  for (int i = 0; i < 7; ++i) c->esdf.counters[i] = h.counts[i];
+  c->esdf.counters[7] = tally.launches;
   c->launches += tally.launches;
   return VBX_OK;
 }

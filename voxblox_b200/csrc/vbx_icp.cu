@@ -340,29 +340,29 @@ int icp_run(vbx_ctx* c, const vbx_icp_config* cfg, const float* points, int on_d
   if (n >= (1ull << 31)) return fail(c, VBX_E_CAPACITY, "icp: too many points");
   const size_t smem = ((size_t)cfg->num_threads * cfg->mini_batch_size * kIcpRec + (size_t)cfg->num_threads * 21) * sizeof(float);
   if (smem > 200 * 1024) return fail(c, VBX_E_CAPACITY, "icp: num_threads * mini_batch_size too large for shared memory");
-  if (n > c->icp_cap || !c->icp_out_dev) {
-    Holdings& h = c->own_icp;
+  if (n > c->icp.cap || !c->icp.out_dev) {
+    Holdings& h = c->icp.own;
     h.release();
-    c->icp_cap = 0;
+    c->icp.cap = 0;
     const uint64_t cap = std::max<uint64_t>(n, 1024);
-    VBX_CUDA(c, h.dev(&c->icp_perm_dev, cap));
-    VBX_CUDA(c, h.host(&c->icp_perm_host, cap));
-    VBX_CUDA(c, h.dev(&c->icp_points_dev, cap * 3));
-    VBX_CUDA(c, h.dev(&c->icp_out_dev, 16));
-    VBX_CUDA(c, h.host(&c->icp_out_host, 16));
-    c->icp_cap = cap;
+    VBX_CUDA(c, h.dev(&c->icp.perm_dev, cap));
+    VBX_CUDA(c, h.host(&c->icp.perm_host, cap));
+    VBX_CUDA(c, h.dev(&c->icp.points_dev, cap * 3));
+    VBX_CUDA(c, h.dev(&c->icp.out_dev, 16));
+    VBX_CUDA(c, h.host(&c->icp.out_host, 16));
+    c->icp.cap = cap;
   }
   cudaStream_t s = c->stream;
   const float* d_points = points;
   if (!on_device && n) {
-    VBX_CUDA(c, cudaMemcpyAsync(c->icp_points_dev, points, n * 3 * sizeof(float), cudaMemcpyHostToDevice, s));
-    d_points = c->icp_points_dev;
+    VBX_CUDA(c, cudaMemcpyAsync(c->icp.points_dev, points, n * 3 * sizeof(float), cudaMemcpyHostToDevice, s));
+    d_points = c->icp.points_dev;
   }
   // the reference's shuffle (icp.cc:229-233) is a function of (n, seed) only: run the C++ library's own
   // std::shuffle on the index sequence while the cloud is on its way to the device
-  std::iota(c->icp_perm_host, c->icp_perm_host + n, 0u);
-  std::shuffle(c->icp_perm_host, c->icp_perm_host + n, std::default_random_engine(seed));
-  if (n) VBX_CUDA(c, cudaMemcpyAsync(c->icp_perm_dev, c->icp_perm_host, n * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+  std::iota(c->icp.perm_host, c->icp.perm_host + n, 0u);
+  std::shuffle(c->icp.perm_host, c->icp.perm_host + n, std::default_random_engine(seed));
+  if (n) VBX_CUDA(c, cudaMemcpyAsync(c->icp.perm_dev, c->icp.perm_host, n * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
 
   IcpParams P;
   P.voxel_size = c->voxel_size;
@@ -386,14 +386,14 @@ int icp_run(vbx_ctx* c, const vbx_icp_config* cfg, const float* points, int on_d
   if (smem > 48 * 1024) {
     VBX_CUDA(c, cudaFuncSetAttribute(k_icp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   }
-  k_icp<<<1, 32 * cfg->num_threads, smem, s>>>(c->tab, P, d_points, c->icp_perm_dev, c->icp_out_dev);
+  k_icp<<<1, 32 * cfg->num_threads, smem, s>>>(c->tab, P, d_points, c->icp.perm_dev, c->icp.out_dev);
   ++c->launches;
   VBX_CUDA(c, cudaGetLastError());
-  VBX_CUDA(c, cudaMemcpyAsync(c->icp_out_host, c->icp_out_dev, 16 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(c->icp.out_host, c->icp.out_dev, 16 * sizeof(float), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));
-  for (int i = 0; i < 4; ++i) out_q[i] = c->icp_out_host[i];
-  for (int i = 0; i < 3; ++i) out_t[i] = c->icp_out_host[4 + i];
-  if (num_updates) *num_updates = *reinterpret_cast<const unsigned long long*>(c->icp_out_host + 8);
+  for (int i = 0; i < 4; ++i) out_q[i] = c->icp.out_host[i];
+  for (int i = 0; i < 3; ++i) out_t[i] = c->icp.out_host[4 + i];
+  if (num_updates) *num_updates = *reinterpret_cast<const unsigned long long*>(c->icp.out_host + 8);
   return VBX_OK;
 }
 

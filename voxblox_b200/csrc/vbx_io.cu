@@ -185,7 +185,7 @@ static const char* layer_type(int layer) { return layer == VBX_LAYER_TSDF ? "tsd
 
 // Layer::saveToFile(file_path, clear_file), core/layer_inl.h:81-157
 int save_layer(vbx_ctx* c, int layer, const char* path, int clear_file) {
-  if (layer == VBX_LAYER_ESDF && !c->has_esdf) return fail(c, VBX_E_STATE, "no ESDF layer");
+  if (layer == VBX_LAYER_ESDF && !c->esdf.ready) return fail(c, VBX_E_STATE, "no ESDF layer");
   const size_t wpv = layer == VBX_LAYER_TSDF ? 3 : 2;
   const size_t wpb = wpv * c->vox_per_block;
   uint64_t n = 0;
@@ -223,7 +223,7 @@ int save_layer(vbx_ctx* c, int layer, const char* path, int clear_file) {
 // io::LoadBlocksFromFile(file_path, kReplace, multiple_layer_support = true, layer), io/layer_io_inl.h:13-90
 int load_layer(vbx_ctx* c, int layer, const char* path, uint64_t* n_loaded) {
   *n_loaded = 0;
-  if (layer == VBX_LAYER_ESDF && !c->has_esdf) return fail(c, VBX_E_STATE, "no ESDF layer");
+  if (layer == VBX_LAYER_ESDF && !c->esdf.ready) return fail(c, VBX_E_STATE, "no ESDF layer");
   FILE* f = std::fopen(path, "rb");
   if (!f) return fail(c, VBX_E_NOT_FOUND, std::string("Could not open protobuf file to load layer: ") + path);
   std::vector<uint8_t> data;

@@ -290,15 +290,13 @@ __global__ void k_mesh_clear_flag(Tables tab, const uint32_t* __restrict__ slots
   if (i < nb) tab.slot_updated[slots[i]] &= (uint8_t)~VBX_UPDATED_MESH;  // block->updated().reset(Update::kMesh), :171-175
 }
 
-static inline unsigned int grid_for(uint64_t n, int block) { return (unsigned int)((n + block - 1) / block); }
-
 // MeshIntegrator::generateMesh(only_mesh_updated_blocks, clear_updated_flag), mesh_integrator.h:132-160
 int mesh_generate(vbx_ctx* c, const vbx_mesh_config* cfg, int only_updated, int clear_flag, uint64_t* n_blocks_out,
                   uint64_t* n_vertices_out) {
   cudaStream_t s = c->stream;
-  c->mesh_idx.clear();
-  c->mesh_first_host.assign(1, 0);
-  c->mesh_use_color = cfg->use_color != 0;
+  c->mesh.idx.clear();
+  c->mesh.first_host.assign(1, 0);
+  c->mesh.use_color = cfg->use_color != 0;
   if (n_blocks_out) *n_blocks_out = 0;
   if (n_vertices_out) *n_vertices_out = 0;
   if (c->n_blocks == 0) return VBX_OK;
@@ -309,24 +307,24 @@ int mesh_generate(vbx_ctx* c, const vbx_mesh_config* cfg, int only_updated, int 
   const std::vector<LayerSlots::Entry> items = view.sorted(VBX_UPDATED_MESH, only_updated ? VBX_UPDATED_MESH : 0);
   if (items.empty()) return VBX_OK;
   const uint32_t nb = (uint32_t)items.size();
-  if (nb > c->mesh_cap_blocks) {
+  if (nb > c->mesh.cap_blocks) {
     const uint64_t want = std::max<uint64_t>(2ull * nb, 256);
-    Holdings& h = c->own_mesh_blocks;
+    Holdings& h = c->mesh.own_blocks;
     h.release();
-    c->mesh_cap_blocks = 0;
-    VBX_CUDA(c, h.dev(&c->mesh_slots, want));
-    VBX_CUDA(c, h.dev(&c->mesh_cube_off, want * c->vox_per_block));
-    VBX_CUDA(c, h.dev(&c->mesh_block_nv, want));
-    VBX_CUDA(c, h.dev(&c->mesh_first, want + 1));
-    c->mesh_cap_blocks = want;
+    c->mesh.cap_blocks = 0;
+    VBX_CUDA(c, h.dev(&c->mesh.slots, want));
+    VBX_CUDA(c, h.dev(&c->mesh.cube_off, want * c->vox_per_block));
+    VBX_CUDA(c, h.dev(&c->mesh.block_nv, want));
+    VBX_CUDA(c, h.dev(&c->mesh.first, want + 1));
+    c->mesh.cap_blocks = want;
   }
   std::vector<uint32_t> slots(nb);
-  c->mesh_idx.resize(3 * (size_t)nb);
+  c->mesh.idx.resize(3 * (size_t)nb);
   for (uint32_t i = 0; i < nb; ++i) {
     slots[i] = items[i].slot;
-    c->mesh_idx[3 * i] = items[i].x;
-    c->mesh_idx[3 * i + 1] = items[i].y;
-    c->mesh_idx[3 * i + 2] = items[i].z;
+    c->mesh.idx[3 * i] = items[i].x;
+    c->mesh.idx[3 * i + 1] = items[i].y;
+    c->mesh.idx[3 * i + 2] = items[i].z;
   }
   MeshParams P;
   P.L = c->L;
@@ -346,36 +344,36 @@ int mesh_generate(vbx_ctx* c, const vbx_mesh_config* cfg, int only_updated, int 
   }
   if ((uint64_t)15 * c->vox_per_block > 0xffffull) return fail(c, VBX_E_CAPACITY, "voxels_per_side too large for 16-bit cube offsets");
   VBX_CUDA(c, cudaEventRecord(c->ev0, s));
-  VBX_CUDA(c, cudaMemcpyAsync(c->mesh_slots, slots.data(), nb * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-  k_mesh_count<<<nb, kMeshThreads, smem, s>>>(P, c->tab, c->mesh_slots, c->mesh_cube_off, c->mesh_block_nv);
+  VBX_CUDA(c, cudaMemcpyAsync(c->mesh.slots, slots.data(), nb * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+  k_mesh_count<<<nb, kMeshThreads, smem, s>>>(P, c->tab, c->mesh.slots, c->mesh.cube_off, c->mesh.block_nv);
   std::vector<uint32_t> nv(nb);
-  VBX_CUDA(c, cudaMemcpyAsync(nv.data(), c->mesh_block_nv, nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  VBX_CUDA(c, cudaMemcpyAsync(nv.data(), c->mesh.block_nv, nb * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   VBX_CUDA(c, cudaStreamSynchronize(s));
   VBX_CUDA(c, cudaGetLastError());
-  c->mesh_first_host.assign((size_t)nb + 1, 0);
-  for (uint32_t i = 0; i < nb; ++i) c->mesh_first_host[i + 1] = c->mesh_first_host[i] + nv[i];
-  const uint64_t total = c->mesh_first_host[nb];
-  if (total > c->mesh_cap_vertices) {
+  c->mesh.first_host.assign((size_t)nb + 1, 0);
+  for (uint32_t i = 0; i < nb; ++i) c->mesh.first_host[i + 1] = c->mesh.first_host[i] + nv[i];
+  const uint64_t total = c->mesh.first_host[nb];
+  if (total > c->mesh.cap_vertices) {
     const uint64_t want = std::max<uint64_t>(total + total / 2, 1u << 16);
-    Holdings& h = c->own_mesh_vertices;
+    Holdings& h = c->mesh.own_vertices;
     h.release();
-    c->mesh_cap_vertices = 0;
-    VBX_CUDA(c, h.dev(&c->mesh_vertices, want * 3));
-    VBX_CUDA(c, h.dev(&c->mesh_normals, want * 3));
-    VBX_CUDA(c, h.dev(&c->mesh_colors, want));
-    c->mesh_cap_vertices = want;
+    c->mesh.cap_vertices = 0;
+    VBX_CUDA(c, h.dev(&c->mesh.vertices, want * 3));
+    VBX_CUDA(c, h.dev(&c->mesh.normals, want * 3));
+    VBX_CUDA(c, h.dev(&c->mesh.colors, want));
+    c->mesh.cap_vertices = want;
   }
   uint64_t launches = 1;
   if (total > 0) {
     static_assert(sizeof(unsigned long long) == sizeof(uint64_t), "first-vertex table");
-    VBX_CUDA(c, cudaMemcpyAsync(c->mesh_first, c->mesh_first_host.data(), ((size_t)nb + 1) * sizeof(uint64_t),
+    VBX_CUDA(c, cudaMemcpyAsync(c->mesh.first, c->mesh.first_host.data(), ((size_t)nb + 1) * sizeof(uint64_t),
                                 cudaMemcpyHostToDevice, s));
-    k_mesh_emit<<<nb, kMeshThreads, smem, s>>>(P, c->tab, c->mesh_slots, c->mesh_cube_off, c->mesh_first, c->mesh_vertices,
-                                               c->mesh_normals, c->mesh_colors);
+    k_mesh_emit<<<nb, kMeshThreads, smem, s>>>(P, c->tab, c->mesh.slots, c->mesh.cube_off, c->mesh.first, c->mesh.vertices,
+                                               c->mesh.normals, c->mesh.colors);
     launches += 1;
   }
   if (clear_flag) {
-    k_mesh_clear_flag<<<grid_for(nb, 256), 256, 0, s>>>(c->tab, c->mesh_slots, nb);
+    k_mesh_clear_flag<<<grid_for(nb, 256), 256, 0, s>>>(c->tab, c->mesh.slots, nb);
     launches += 1;
   }
   VBX_CUDA(c, cudaEventRecord(c->ev1, s));
@@ -383,7 +381,6 @@ int mesh_generate(vbx_ctx* c, const vbx_mesh_config* cfg, int only_updated, int 
   VBX_CUDA(c, cudaGetLastError());
   VBX_CUDA(c, cudaEventElapsedTime(&c->last_ms, c->ev0, c->ev1));
   c->launches += launches;
-  c->mesh_launches = launches;
   if (n_blocks_out) *n_blocks_out = nb;
   if (n_vertices_out) *n_vertices_out = total;
   return VBX_OK;
@@ -392,16 +389,16 @@ int mesh_generate(vbx_ctx* c, const vbx_mesh_config* cfg, int only_updated, int 
 // the result of the last mesh_generate, block by block in index order
 int mesh_download(vbx_ctx* c, int32_t* idx3, uint64_t* first_vertex, float* vertices, float* normals, uint8_t* colors) {
   cudaStream_t s = c->stream;
-  const size_t nb = c->mesh_idx.size() / 3;
-  if (idx3 && nb) std::memcpy(idx3, c->mesh_idx.data(), nb * 3 * sizeof(int32_t));
-  if (first_vertex) std::memcpy(first_vertex, c->mesh_first_host.data(), c->mesh_first_host.size() * sizeof(uint64_t));
-  const uint64_t total = c->mesh_first_host.back();
+  const size_t nb = c->mesh.idx.size() / 3;
+  if (idx3 && nb) std::memcpy(idx3, c->mesh.idx.data(), nb * 3 * sizeof(int32_t));
+  if (first_vertex) std::memcpy(first_vertex, c->mesh.first_host.data(), c->mesh.first_host.size() * sizeof(uint64_t));
+  const uint64_t total = c->mesh.first_host.back();
   if (total == 0) return VBX_OK;
-  if (vertices) VBX_CUDA(c, cudaMemcpyAsync(vertices, c->mesh_vertices, total * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
-  if (normals) VBX_CUDA(c, cudaMemcpyAsync(normals, c->mesh_normals, total * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if (vertices) VBX_CUDA(c, cudaMemcpyAsync(vertices, c->mesh.vertices, total * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if (normals) VBX_CUDA(c, cudaMemcpyAsync(normals, c->mesh.normals, total * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
   if (colors) {
-    if (!c->mesh_use_color) return fail(c, VBX_E_STATE, "the last mesh was generated without colours");
-    VBX_CUDA(c, cudaMemcpyAsync(colors, c->mesh_colors, total * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    if (!c->mesh.use_color) return fail(c, VBX_E_STATE, "the last mesh was generated without colours");
+    VBX_CUDA(c, cudaMemcpyAsync(colors, c->mesh.colors, total * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   }
   VBX_CUDA(c, cudaStreamSynchronize(s));
   return VBX_OK;

@@ -2010,8 +2010,6 @@ int init_bundle_order(vbx_ctx* c) {
   return VBX_OK;
 }
 
-static inline unsigned int grid_for(uint64_t n, int block) { return (unsigned int)((n + block - 1) / block); }
-
 int check_state_errors(vbx_ctx* c, const ScanState& h) {
   const uint32_t err = h.error & kFatalErrors;
   if (!err) return VBX_OK;
@@ -2586,12 +2584,12 @@ void report_scan(vbx_ctx* c, const ScanState& h, int kind, uint64_t launches, ui
 // sms: the grid unit of the graph's kernels.
 static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& F, const ScanParams& P,
                         vbx_ctx::ScanGraph& G, unsigned int sms) {
-  const int k = (int)(&S - c->set), sets = c->sets_in_use;
+  const int k = (int)(&S - c->set), sets = c->pipe.sets_in_use;
   const vbx_ctx::ScratchSet& prev = c->set[(k + sets - 1) % sets];
   const vbx_ctx::ScratchSet& prev2 = c->set[(k + 2 * sets - 2) % sets];
-  const Capture cap{c->stream_s, c->stream, S.walked, S.sorted, S.applied, prev2.sorted, prev.applied,
-                    {c->cap_ev[2], c->cap_ev[3]}};
-  const ScanRoute front{S, F, F.stream, sms, false}, walk{S, F, c->stream_e, sms, false};
+  const Capture cap{c->pipe.stream_s, c->stream, S.walked, S.sorted, S.applied, prev2.sorted, prev.applied,
+                    {c->pipe.cap_ev[2], c->pipe.cap_ev[3]}};
+  const ScanRoute front{S, F, F.stream, sms, false}, walk{S, F, c->pipe.stream_e, sms, false};
   cudaStream_t o = S.stream;
   Tally tally{c, F.stream, false};  // (the graph's kernel nodes are counted below)
   auto enqueue = [&]() -> int {
@@ -2599,29 +2597,29 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
     VBX_CUDA(c, cudaStreamWaitEvent(o, S.copy_done, cudaEventWaitExternal));  // a host cloud's copy
     VBX_CUDA(c, cudaStreamWaitEvent(o, F.done, cudaEventWaitExternal));       // the lane's previous front half
     // ---- front half on the lane's stream
-    VBX_CUDA(c, cudaEventRecord(c->cap_ev[0], o));
-    VBX_CUDA(c, cudaStreamWaitEvent(F.stream, c->cap_ev[0], 0));
+    VBX_CUDA(c, cudaEventRecord(c->pipe.cap_ev[0], o));
+    VBX_CUDA(c, cudaStreamWaitEvent(F.stream, c->pipe.cap_ev[0], 0));
     VBX_CUDA(c, cudaMemsetAsync(S.d_state, 0, sizeof(ScanState), F.stream));
-    if (c->timeline) VBX_CUDA(c, cudaEventRecordWithFlags(S.front_start, F.stream, cudaEventRecordExternal));
+    if (c->pipe.timeline) VBX_CUDA(c, cudaEventRecordWithFlags(S.front_start, F.stream, cudaEventRecordExternal));
     if (int rc = front_half(c, front, P, nullptr, tally)) return rc;
     VBX_CUDA(c, cudaEventRecordWithFlags(F.done, F.stream, cudaEventRecordExternal));
-    if (c->timeline) VBX_CUDA(c, cudaEventRecordWithFlags(S.front_done, F.stream, cudaEventRecordExternal));
+    if (c->pipe.timeline) VBX_CUDA(c, cudaEventRecordWithFlags(S.front_done, F.stream, cudaEventRecordExternal));
     // ---- walk, record sort and apply (sort_and_apply hands off between their streams)
-    VBX_CUDA(c, cudaEventRecord(c->cap_ev[1], F.stream));
-    VBX_CUDA(c, cudaStreamWaitEvent(c->stream_e, c->cap_ev[1], 0));
-    VBX_CUDA(c, cudaStreamWaitEvent(c->stream_e, prev.walked, cudaEventWaitExternal));
+    VBX_CUDA(c, cudaEventRecord(c->pipe.cap_ev[1], F.stream));
+    VBX_CUDA(c, cudaStreamWaitEvent(c->pipe.stream_e, c->pipe.cap_ev[1], 0));
+    VBX_CUDA(c, cudaStreamWaitEvent(c->pipe.stream_e, prev.walked, cudaEventWaitExternal));
     // Scans run their map-touching stages in submission order.  A scan that cannot be applied
     // asynchronously (more update records than one pass holds) raises the context's hold flag here;
     // every scan queued behind it then skips its back half, and the host redoes all of them
     // synchronously, in order, from the retained inputs (recover_async, vbx_capi.cu).
-    k_back_begin<<<1, 1, 0, c->stream_e>>>(S.d_state, c->d_hold);
+    k_back_begin<<<1, 1, 0, c->pipe.stream_e>>>(S.d_state, c->pipe.d_hold);
     if (int rc = back_half(c, walk, tally, &cap)) return rc;
     VBX_CUDA(c, cudaMemcpyAsync(S.h_state, S.d_state, sizeof(ScanState), cudaMemcpyDeviceToHost, cap.apply));
     // every stream of the capture joins its origin
-    const cudaStream_t joined[4] = {F.stream, c->stream_e, c->stream_s, c->stream};
+    const cudaStream_t joined[4] = {F.stream, c->pipe.stream_e, c->pipe.stream_s, c->stream};
     for (int j = 0; j < 4; ++j) {
-      VBX_CUDA(c, cudaEventRecord(c->cap_ev[4 + j], joined[j]));
-      VBX_CUDA(c, cudaStreamWaitEvent(o, c->cap_ev[4 + j], 0));
+      VBX_CUDA(c, cudaEventRecord(c->pipe.cap_ev[4 + j], joined[j]));
+      VBX_CUDA(c, cudaStreamWaitEvent(o, c->pipe.cap_ev[4 + j], 0));
     }
     return VBX_OK;
   };
@@ -2692,7 +2690,7 @@ static int capture_scan(vbx_ctx* c, vbx_ctx::ScratchSet& S, vbx_ctx::FrontLane& 
   if (rc != VBX_OK) return rc;
   G.graph = std::exchange(g, nullptr);
   G.exec = std::exchange(x, nullptr);
-  c->own_async.graph(&G.graph, &G.exec);
+  c->pipe.own.graph(&G.graph, &G.exec);
   G.launches = launches;
   G.point_sort = point_sort;
   G.point_grid = pp.gridDim.x;
@@ -2766,13 +2764,13 @@ int integrate_async(vbx_ctx* c, const ScanRoute& sync, int kind, const float q[4
   }
   if (int rc = ensure_async(c)) return rc;
   const uint32_t n = (uint32_t)n64;
-  const int k = (int)(c->async_seq % c->sets_in_use);
-  const int l = (int)(c->async_seq % c->lanes_in_use);
+  const int k = (int)(c->pipe.seq % c->pipe.sets_in_use);
+  const int l = (int)(c->pipe.seq % c->pipe.lanes_in_use);
   vbx_ctx::ScratchSet& S = c->set[k];
   const auto t_enter = std::chrono::steady_clock::now();
   if (S.in_flight) {  // bounded run-ahead: wait for the scan that used this hand-off set
     VBX_CUDA(c, cudaEventSynchronize(S.back_done));
-    c->async_wait_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t_enter).count();
+    c->pipe.wait_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t_enter).count();
     harvest_async(c, S);
     if (S.redo) {
       // it (and every scan queued behind it) did not run its back half: redo them now, in order
@@ -2786,7 +2784,7 @@ int integrate_async(vbx_ctx* c, const ScanRoute& sync, int kind, const float q[4
   if (!on_device) {
     // the copy engine works ahead of the front half on a stream of its own
     // (two copy streams alternate, so two scans' clouds can be in flight on the copy engines at once)
-    cudaStream_t sc = (c->async_seq & 1u) ? c->stream_c2 : c->stream_c;
+    cudaStream_t sc = (c->pipe.seq & 1u) ? c->stream_c2 : c->stream_c;
     if (cudaMemcpyAsync(S.d_xyz, xyz, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, sc) != cudaSuccess ||
         cudaMemcpyAsync(S.d_rgba, rgba, (size_t)n * 4, cudaMemcpyHostToDevice, sc) != cudaSuccess ||
         cudaEventRecord(S.copy_done, sc) != cudaSuccess) {
@@ -2808,9 +2806,9 @@ int integrate_async(vbx_ctx* c, const ScanRoute& sync, int kind, const float q[4
   if (!G.exec) {
     // the first scan of its kind captures the graphs of every (set, lane) pair the submission order
     // reaches (set = seq % sets, lane = seq % lanes), so that no later scan waits for a capture
-    const int pairs = std::lcm(c->sets_in_use, c->lanes_in_use);
+    const int pairs = std::lcm(c->pipe.sets_in_use, c->pipe.lanes_in_use);
     for (int j = 0; j < pairs && rc == VBX_OK; ++j) {
-      const int kj = j % c->sets_in_use, lj = j % c->lanes_in_use;
+      const int kj = j % c->pipe.sets_in_use, lj = j % c->pipe.lanes_in_use;
       rc = capture_scan(c, c->set[kj], c->lane[lj], P, c->set[kj].graph[lj][variant], sms);
     }
   }
@@ -2823,7 +2821,7 @@ int integrate_async(vbx_ctx* c, const ScanRoute& sync, int kind, const float q[4
   S.in_flight = true;
   S.kind = kind;
   S.launches = G.launches;
-  S.seq = c->async_seq;
+  S.seq = c->pipe.seq;
   S.redo = false;
   std::memcpy(S.q, q, sizeof(S.q));
   std::memcpy(S.t, t, sizeof(S.t));
@@ -2831,13 +2829,13 @@ int integrate_async(vbx_ctx* c, const ScanRoute& sync, int kind, const float q[4
   S.freespace = freespace;
   S.in_xyz = dx;   // (the set's private copy of a host cloud, or the caller's device buffers)
   S.in_rgba = dr;
-  c->async_submit_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t_enter).count();
+  c->pipe.submit_ns += (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t_enter).count();
   c->launches += G.launches;
-  c->async_seq += 1;
-  if (c->deferred_rc) {
-    rc = c->deferred_rc;
-    c->err = c->deferred_msg;
-    c->deferred_rc = 0;
+  c->pipe.seq += 1;
+  if (c->pipe.deferred_rc) {
+    rc = c->pipe.deferred_rc;
+    c->err = c->pipe.deferred_msg;
+    c->pipe.deferred_rc = 0;
     return rc;
   }
   return VBX_OK;
